@@ -1,4 +1,4 @@
-"""Drop-in ``MinkowskiEngine`` for OpenScene, backed by libosb200 (B200 / sm_100a).
+"""Drop-in ``MinkowskiEngine`` for OpenScene, backed by libosb200 (H100 / sm_90a).
 
 ``import MinkowskiEngine as ME`` in the reference's models/mink_unet.py:25, models/resnet_base.py:27,
 run/distill.py:18 and run/evaluate.py:18 resolves here when this repository is on PYTHONPATH.

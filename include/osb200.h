@@ -1,5 +1,5 @@
 /*
- * osb200.h -- C ABI of libosb200.so, the B200 (sm_100a) sparse-3D-convolution + open-vocabulary
+ * osb200.h -- C ABI of libosb200.so, the H100 (sm_90a) sparse-3D-convolution + open-vocabulary
  * matching engine that replaces the MinkowskiEngine native backend and the driver-side torch ops on
  * OpenScene's hot path.
  *
@@ -35,7 +35,7 @@
  *     tuning knobs of osb_tuning_set, which never change results);
  *   - every function returns 0 on success, non-zero on failure; osb_last_error() returns a
  *     thread-local description; no exception crosses the ABI;
- *   - there is no CPU fallback: on a machine without an sm_100 GPU every compute entry point fails.
+ *   - there is no CPU fallback: on a machine without an sm_90 GPU every compute entry point fails.
  */
 #ifndef OSB200_H
 #define OSB200_H
@@ -138,7 +138,7 @@ size_t osb_conv_wgrad_tc_workspace_bytes(int64_t n_out, int32_t K, int32_t cin, 
 int osb_conv_wgrad_tc(const void *x_split, int32_t cin, int64_t n_in, const int32_t *nbr, int64_t n_out, int32_t K,
                       const void *gout_split, int32_t cout, float *gw, void *ws, size_t ws_bytes, void *stream);
 
-/* Tensor-core path (tcgen05, bf16x3 split-fp32 operands, fp32 accumulation in TMEM).
+/* Tensor-core path (wgmma, bf16x3 split-fp32 operands, fp32 accumulation in registers).
  *
  * Activation "split" layout: a row of C channels (C % 32 == 0) is 4*C bytes; every 32-channel block is
  * one 128-byte line [bf16 hi x32 | bf16 lo x32] with hi = bf16_rn(v), lo = bf16_rn(v - hi).
@@ -155,7 +155,7 @@ int osb_conv_wgrad_tc(const void *x_split, int32_t cin, int64_t n_in, const int3
  *   out_split   split rows [n_out, cout] or NULL
  *   out_f32     fp32 [n_out, cout] or NULL; out_row_map (int32 [n_out] or NULL) scatters fp32 rows:
  *               row o is written to out_f32[out_row_map[o]]
- *   flags       bit0: launch with programmatic stream serialization (PDL).  The kernel's prologue (barrier / TMEM
+ *   flags       bit0: launch with programmatic stream serialization (PDL).  The kernel's prologue (barrier
  *               set-up, loading `nbr`, scale, shift) then overlaps the tail of the previous kernel in `stream`; it
  *               waits for that kernel before touching src*, res, ws or any output.  Only legal when nbr / wpack /
  *               scale / shift were NOT produced by the immediately preceding kernel in the stream.
@@ -184,7 +184,7 @@ int osb_convtr_fwd_tc(const void *src, int32_t cin, int64_t n_coarse, const int3
 /* ----------------------------------------------------------- persistent convolution chains (conv_chain.cu)
  * Second-generation tensor-core path: ONE launch executes a list of convolution layers (`MinkowskiConvolution` /
  * `MinkowskiConvolutionTranspose` forwards of consecutive modules of models/mink_unet.py:116-174, BasicBlock included) with
- * one persistent CTA per SM, dedicated epilogue warps, a double-buffered TMEM accumulator, split-K reduced inside the
+ * one persistent CTA per SM, producer warps and two consumer warpgroups (wgmma + epilogue), split-K reduced inside the
  * kernel and grid barriers between dependent layers.  Same arithmetic and the same argument meaning as osb_conv_fwd_tc.
  *
  * A layer is described by an opaque record of osb_conv_desc_bytes() bytes, filled on the HOST by osb_conv_desc_fill; the

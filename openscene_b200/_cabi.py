@@ -75,7 +75,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"openscene_b200: native library {LIB_PATH} is missing. Build it with "
-                f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+                f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
                 f"There is no CPU/PyTorch fallback for this path.")
         L = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():

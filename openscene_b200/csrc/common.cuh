@@ -1,4 +1,4 @@
-// Shared helpers for libosb200 (sm_100a only).
+// Shared helpers for libosb200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

@@ -1,31 +1,29 @@
-// Persistent, plan-driven sparse convolution on 5th-gen tensor cores (second generation of conv_tc.cu).
+// Persistent, plan-driven sparse convolution on tensor cores (wgmma; second generation of conv_tc.cu).
 //
 //   out[o,:] = epilogue( sum_k  in[nbr[k][o], :] @ W[k] )         (output-stationary, no atomics)
 //
-// One launch executes a LIST of convolution layers ("chain") described by ConvDesc records in device memory.  The grid
-// is one CTA per SM; every CTA owns a contiguous range of each layer's work units (unit = 128 output rows x one N tile x
+// One launch executes a LIST of convolution layers ("chain") described by ConvDesc records passed as kernel parameters.  The
+// grid is one CTA per SM; every CTA owns a contiguous range of each layer's work units (unit = 128 output rows x one N tile x
 // one split of the (offset, channel-block) stage sequence) and walks it with warp-specialised roles that never leave
 // their loops between units:
 //
-//   warps 0-3   epilogue of both TMEM accumulator buffers: TMEM -> registers -> BN affine / residual / ReLU -> swizzled
-//               staging tile -> full-line coalesced stores (split rows, fp32 rows, or raw split-K partials)
-//   warp 4      weight tiles: one cp.async.bulk per stage from the tile-major, pre-swizzled packing (no tensor map)
-//   warps 5-6   tcgen05.mma issuers (one thread each): warp 5 owns sub-tile 0 of an item, warp 6 sub-tile 1; warp 5 owns TMEM
-//   warps 8-15  gathered A rows: cp.async 16 B x 8 lanes per 128-byte row line, hand-applied 128B swizzle, the kernel
-//               map read per offset straight from global memory, one offset ahead
+//   warp 0       weight tiles: one cp.async.bulk per stage from the tile-major, pre-swizzled packing (no tensor map)
+//   warps 1-3    gathered A rows: cp.async 16 B x 8 lanes per 128-byte row line, hand-applied 128B swizzle, the kernel
+//                map read per offset straight from global memory, one slot of the warp ahead
+//   warps 4-11   two consumer warpgroups: warpgroup g multiplies rows [64g, 64g+64) of every sub-tile of an item (wgmma,
+//                accumulators in registers), then runs the epilogue on them: BN affine / residual / ReLU -> swizzled
+//                staging tile -> full-line coalesced stores (split rows, fp32 rows, or raw split-K partials)
 //
-// What changed against conv_tc.cu, and why (profiles/r01_ncu_full_conv_tc_96x96_k3_final.md, DESIGN.md "slot model"):
-//   * separate rings for gathered rows and weight tiles; the whole SM's shared memory belongs to one CTA: 9-10 row
-//     slots of 16 KB in flight per SM instead of 6 (the stage rate was latency x row bytes in flight);
-//   * two 128-row sub-tiles share every weight tile (256 output rows per item): half the L2->SM weight stream;
-//   * the accumulator is double buffered in TMEM (2 x 256 columns) and drained by dedicated epilogue warps while the
-//     next item's MMAs run; barrier / TMEM set-up is paid once per CTA, not once per tile; work is split evenly over
-//     the SMs (no 6-vs-5.2 wave tail);
+// Against conv_tc.cu:
+//   * separate rings for gathered rows and weight tiles; the whole SM's shared memory belongs to one CTA;
+//   * two 128-row sub-tiles share every weight tile (256 output rows per item) for N tiles of at most CH_MAX_PAIR_NT
+//     columns: half the L2->SM weight stream;
+//   * barrier set-up is paid once per CTA, not once per tile; work is split evenly over the SMs (no wave tail);
 //   * split-K partials are reduced INSIDE the kernel after a grid barrier, and consecutive small layers (levels 2-4 of
 //     the U-Net) run in one launch with grid barriers between dependent layers: no launch / finish-kernel boundaries.
 //
-// Numerics are those of conv_tc.cu: split-bf16 operands (v = hi + lo), hi*Whi + hi*Wlo + lo*Whi on kind::f16 MMAs,
-// fp32 accumulation in TMEM, deterministic (fixed-order) split-K reduction.
+// Numerics are those of conv_tc.cu: split-bf16 operands (v = hi + lo), hi*Whi + hi*Wlo + lo*Whi on bf16 wgmma,
+// fp32 accumulation, deterministic (fixed-order) split-K reduction.
 #include "tc_ptx.cuh"
 #include <algorithm>
 #include <cstring>
@@ -33,21 +31,19 @@
 
 namespace osb {
 
-constexpr int CH_THREADS = 384;                  // 12 warps (3 per scheduler -> 168 registers each): 4 epilogue, 1 weights, 2 MMA issuers, 5 gather
-constexpr int CH_M = 128;                        // rows per sub-tile (UMMA M)
+constexpr int CH_THREADS = 384;                  // 12 warps (168 registers each): 1 weights, 3 gather, 2 consumer warpgroups
+constexpr int CH_M = 128;                        // rows per sub-tile
 constexpr int CH_A_BYTES = CH_M * 128;           // one row slot: 128 rows x one 32-channel block
-constexpr int CH_STG_BYTES = 4 * 4096;           // epilogue staging: 4 warps x (32 rows x 128 B)
+constexpr int CH_STG_BYTES = 8 * 2048;           // epilogue staging: 8 consumer warps x (16 rows x 128 B)
 constexpr int CH_SS_FLOATS = 768;                // folded BN constants kept in shared memory per layer (scale | shift)
 constexpr int CH_MAX_SA = 12, CH_MAX_SB = 4;
-// Warp roles.  Measured with per-role cycle counters (profiles/r02_chain_roles.md): every role is ONE warp walking a
-// dependent instruction chain, so its fixed cost per row slot (barrier wait, address set-up, arrival: 300-500 cycles) is
-// latency, not throughput.  Gather producers therefore own whole slots (ring slot s is always filled by warp s mod CH_A_WARPS, 32 copy
-// instructions behind one wait / one arrival), the epilogue (idle 90 % of the time) gets four warps for both TMEM buffers.
-constexpr int CH_W_EPI = 0;                       // warps 0-3: epilogue (warp % 4 = TMEM lane quarter), both accumulator buffers
-constexpr int CH_W_B = 4;                         // weight tiles
-constexpr int CH_W_MMA = 5;                       // warps 5, 6: MMA issuers; warp 5 owns the TMEM allocation
-constexpr int CH_W_A = 7;                         // warps 7-11: gathered rows, one whole 128-row slot at a time each
-constexpr int CH_A_WARPS = 5;
+// Warp roles.  Every producer role is ONE warp walking a dependent instruction chain, so its fixed cost per row slot
+// (barrier wait, address set-up, arrival) is latency, not throughput.  Gather producers therefore own whole slots (ring slot
+// s is always filled by warp s mod CH_A_WARPS, 32 copy instructions behind one wait / one arrival).
+constexpr int CH_W_B = 0;                         // weight tiles
+constexpr int CH_W_A = 1;                         // warps 1-3: gathered rows, one whole 128-row slot at a time each
+constexpr int CH_A_WARPS = 3;
+constexpr int CH_W_MMA = 4;                       // warps 4-11: two consumer warpgroups (wgmma + epilogue)
 constexpr int CH_DESC_WORDS = 48;                // sizeof(ConvDesc) / 4
 constexpr int CH_MAX_LAYERS = 16;                // layers per launch: the descriptors travel as kernel parameters (3 KB)
 
@@ -66,15 +62,14 @@ struct __align__(16) ConvDesc {
   int K, nb0, nb1;
   int cout, cout_pad, nt, n_ntiles;
   int relu, cmap_cout, nsplit, m_tiles;
-  int nsub_max;                    // sub-tiles per item that may share a weight tile: 2 when nt <= 128, else 1
+  int nsub_max;                    // sub-tiles per item that may share a weight tile: 2 when nt <= CH_MAX_PAIR_NT, else 1
   int barrier_before;              // grid barrier before this layer (it reads what an earlier layer of the launch wrote)
   int stages_per_split;            // ceil(K * (nb0 + nb1) / nsplit)
   int pad[8];
 };
 static_assert(sizeof(ConvDesc) == CH_DESC_WORDS * 4, "ConvDesc layout");
 // The layer list lives in the kernel's parameter (constant) space: every field is a warp-uniform value to the compiler, so
-// the single-thread roles (MMA issuers, weight producer) keep their slot / descriptor arithmetic on the uniform datapath
-// instead of paying vector->uniform register moves in front of every tcgen05.mma (profiles/r02_chain_roles.md).
+// the roles keep their slot / descriptor arithmetic on the uniform datapath.
 struct ChainArgs { ConvDesc d[CH_MAX_LAYERS]; };
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
@@ -166,10 +161,6 @@ __device__ __forceinline__ void grid_barrier(unsigned *gbar, unsigned &gen) {
   __syncthreads();
 }
 
-// per-role cycle accounting (tuning; active only when a clock buffer is given): dbg_clock[cta*32 + slot]
-#define CH_PROF_BEGIN() const long long _t0 = prof ? clock64() : 0
-#define CH_PROF_END(var) do { if (prof) var += clock64() - _t0; } while (0)
-
 // keep a value in its register: stops the compiler from re-deriving shared-window addresses (S2R + shifts) in hot loops
 #define CH_KEEP(x) asm volatile("" : "+r"(x))
 
@@ -181,6 +172,132 @@ __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void *src, 
       "cp.async.cg.shared.global [%0], [%1], 16, p;\n\t}"
       ::"r"(dst), "l"(src), "r"(ignore)
       : "memory");
+}
+
+// ------------------------------------------------------------------------------------ consumer: one item
+// Rings and barriers of the CTA, as a consumer warpgroup sees them.
+struct ChainRings {
+  uint32_t a_ring, b_ring, bslot, sa, sb;
+  uint32_t fullA, emptyA, fullB, emptyB;
+};
+
+// One item of consumer warpgroup g: rows [64g, 64g+64) of NSUB 128-row sub-tiles sharing each weight tile, N = 32 NCH
+// columns, stages [t_begin, t_end).  Compile-time shapes keep the accumulators a fixed register set and every wgmma of a
+// stage branch-free, so a stage's wgmmas stay in flight while the next stage's barriers are awaited; its slots are released
+// one stage later (after wgmma_wait<1>).  Sub-tile s, 32-column block c accumulates in acc[16 (NCH s + c) ..].
+template <int NCH, int NSUB>
+__device__ __forceinline__ void chain_item(const ChainRings &R, const ConvDesc &E, const float *s_ss, uint32_t stgw, bool no_store,
+                                           uint32_t &a_slot_io, uint32_t &a_phase_io,
+                                        uint32_t &b_slot_io, uint32_t &b_phase_io, int t_begin, int t_end, int z, int nti, int m,
+                                        int g, int warp, int lane) {
+  float acc[NSUB * NCH * 16];
+#pragma unroll
+  for (int i = 0; i < NSUB * NCH * 16; ++i) acc[i] = 0.f;
+  const bool leader = (threadIdx.x & 127) == 0;
+  uint32_t a_slot = a_slot_io, a_phase = a_phase_io, b_slot = b_slot_io, b_phase = b_phase_io;   // ring positions, in registers
+  uint32_t pa0 = 0, pa1 = 0, pb = 0;                 // slots of the previous stage, to release
+  for (int t = t_begin; t < t_end; ++t) {
+    uint32_t a1 = a_slot + 1u, ap1 = a_phase;
+    if (a1 >= R.sa) { a1 -= R.sa; ap1 ^= 1u; }
+    for (uint32_t it = 0;; ++it) {                   // all barriers of the stage probed together (overlapping round trips)
+      uint32_t ok = mbar_try(R.fullB + 8 * b_slot, b_phase) & mbar_try(R.fullA + 8 * a_slot, a_phase);
+      if (NSUB == 2) ok &= mbar_try(R.fullA + 8 * a1, ap1);
+      if (ok) break;
+      if (it > (1u << 26)) __trap();
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) writes -> wgmma reads
+    const uint64_t db = gmma_desc(R.b_ring + b_slot * R.bslot);
+    wgmma_fence();
+    wg_split_mma<NCH>(acc, gmma_desc(R.a_ring + a_slot * (uint32_t)CH_A_BYTES + (uint32_t)g * 64u * 128u), db);
+    if (NSUB == 2) wg_split_mma<NCH>(acc + NCH * 16, gmma_desc(R.a_ring + a1 * (uint32_t)CH_A_BYTES + (uint32_t)g * 64u * 128u), db);
+    wgmma_commit();
+    wgmma_wait<1>();                                  // the previous stage's wgmmas have retired: release its slots
+    if (leader && t > t_begin) {
+      mbar_arrive(R.emptyA + 8 * pa0);
+      if (NSUB == 2) mbar_arrive(R.emptyA + 8 * pa1);
+      mbar_arrive(R.emptyB + 8 * pb);
+    }
+    pa0 = a_slot; pa1 = a1; pb = b_slot;
+    a_slot += (uint32_t)NSUB;
+    if (a_slot >= R.sa) { a_slot -= R.sa; a_phase ^= 1u; }
+    if (++b_slot == R.sb) { b_slot = 0; b_phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_hold(acc);
+  a_slot_io = a_slot; a_phase_io = a_phase; b_slot_io = b_slot; b_phase_io = b_phase;
+  if (leader && t_end > t_begin) {
+    mbar_arrive(R.emptyA + 8 * pa0);
+    if (NSUB == 2) mbar_arrive(R.emptyA + 8 * pa1);
+    mbar_arrive(R.emptyB + 8 * pb);
+  }
+  // ---- epilogue of this warp's 16 rows of every sub-tile, one 32-column block at a time
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int s = 0; s < NSUB; ++s) {
+    const int64_t wrow0 = (int64_t)(m + s) * CH_M + 64 * g + 16 * (warp & 3);   // first global row of this warp
+    auto plain_row = [&](int r) -> int64_t { return (!no_store && wrow0 + r < E.n_out) ? wrow0 + r : -1; };
+#pragma unroll
+    for (int cbo = 0; cbo < NCH; ++cbo) {
+      float *y = acc + 16 * (NCH * s + cbo);
+      const int c0 = nti * E.nt + cbo * 32;           // first output channel of this 32-block
+      if (E.nsplit > 1) {                             // raw partial sums; the reduce phase applies the epilogue
+        frag_stage_f32(stgw, y, lane);
+        __syncwarp();
+        stage_flush(stgw, reinterpret_cast<uint8_t *>(E.partial + (int64_t)z * E.n_out * E.cout_pad), (int64_t)E.cout_pad * 4,
+                    (int64_t)c0 * 4, lane, plain_row);
+        __syncwarp();
+        continue;
+      }
+      if (c0 >= E.cout) continue;                     // warp-uniform (padding columns)
+      int oc0 = c0, out_c = E.cout, kch = 0;
+      if (E.cmap) {                                   // dense transposed conv: this column block belongs to child kch
+        kch = c0 / E.cmap_cout;
+        oc0 = c0 - kch * E.cmap_cout;
+        out_c = E.cmap_cout;
+      }
+      if (E.scale) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int col = oc0 + 8 * i + cq + (e & 1);
+            y[4 * i + e] = fmaf(y[4 * i + e], s_ss[col], s_ss[CH_SS_FLOATS + col]);
+          }
+      }
+      if (E.res) {                                    // residual tile: coalesced load -> staging -> own fragment
+        stage_load(stgw, E.res, wrow0, E.n_out, (int64_t)E.cout * 4, (int64_t)(c0 >> 5) * 128, lane);
+        __syncwarp();
+        frag_add_split(stgw, y, lane);
+        __syncwarp();
+      }
+      if (E.relu) {
+#pragma unroll
+        for (int e = 0; e < 16; ++e) y[e] = fmaxf(y[e], 0.f);
+      }
+      auto cmap_row = [&](int r) -> int64_t {
+        return (!no_store && wrow0 + r < E.n_out) ? (int64_t)__ldg(E.cmap + (int64_t)kch * E.n_out + wrow0 + r) : -1;
+      };
+      if (E.out_split) {
+        frag_stage_split(stgw, y, lane);
+        __syncwarp();
+        if (E.cmap) stage_flush(stgw, E.out_split, (int64_t)out_c * 4, (int64_t)(oc0 >> 5) * 128, lane, cmap_row);
+        else stage_flush(stgw, E.out_split, (int64_t)out_c * 4, (int64_t)(oc0 >> 5) * 128, lane, plain_row);
+        __syncwarp();
+      }
+      if (E.out_f32) {
+        frag_stage_f32(stgw, y, lane);
+        __syncwarp();
+        uint8_t *base = reinterpret_cast<uint8_t *>(E.out_f32);
+        if (E.cmap) stage_flush(stgw, base, (int64_t)out_c * 4, (int64_t)oc0 * 4, lane, cmap_row);
+        else if (E.out_row_map)
+          stage_flush(stgw, base, (int64_t)out_c * 4, (int64_t)oc0 * 4, lane, [&](int r) -> int64_t {
+            return (!no_store && wrow0 + r < E.n_out) ? (int64_t)__ldg(E.out_row_map + wrow0 + r) : -1;
+          });
+        else stage_flush(stgw, base, (int64_t)out_c * 4, (int64_t)oc0 * 4, lane, plain_row);
+        __syncwarp();
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------ the kernel
@@ -195,47 +312,36 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
   uint8_t *smem = smem_raw + (base_u32 - raw_u32);
   const uint32_t a_ring = base_u32;                                          // row slots
   const uint32_t b_ring = a_ring + (uint32_t)sa * CH_A_BYTES;                // weight slots (bslot is a multiple of 1024)
-  const uint32_t stg_u32 = b_ring + (uint32_t)sb * (uint32_t)bslot;          // epilogue staging: 4 warps x 4 KB
+  const uint32_t stg_u32 = b_ring + (uint32_t)sb * (uint32_t)bslot;          // epilogue staging: 8 warps x 2 KB
   uint32_t a_ring_k = a_ring, b_ring_k = b_ring;
   CH_KEEP(a_ring_k); CH_KEEP(b_ring_k);
   uint8_t *aux = smem + (stg_u32 - base_u32) + CH_STG_BYTES;
   float *s_ss = reinterpret_cast<float *>(aux);                              // [scale x CH_SS_FLOATS | shift x CH_SS_FLOATS]
   uint64_t *bars = reinterpret_cast<uint64_t *>(s_ss + 2 * CH_SS_FLOATS);
-  uint32_t *s_misc = reinterpret_cast<uint32_t *>(bars + 40);                // [0] TMEM base
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (flags & 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  const bool prof = dbg_clock != nullptr;
-  long long pw0 = 0, pw1 = 0, pw2 = 0, pt = 0;     // cycles in this role's waits (up to three kinds) and in its loop
   if (dbg_clock && tid == 0) dbg_clock[blockIdx.x * 32 + 0] = clock64();
   uint32_t fullA = smem_u32(bars), emptyA = fullA + 12 * 8, fullB = fullA + 24 * 8, emptyB = fullA + 28 * 8;
-  uint32_t accFull = fullA + 32 * 8, accEmpty = fullA + 34 * 8;
-  CH_KEEP(fullA); CH_KEEP(emptyA); CH_KEEP(fullB); CH_KEEP(emptyB); CH_KEEP(accFull); CH_KEEP(accEmpty);
+  CH_KEEP(fullA); CH_KEEP(emptyA); CH_KEEP(fullB); CH_KEEP(emptyB);
 
   if (tid == 0) {
-    for (int s = 0; s < sa; ++s) { mbar_init(fullA + 8 * s, 32); mbar_init(emptyA + 8 * s, 1); }   // fullA: the 32 lanes of the slot's warp
-    for (int s = 0; s < sb; ++s) { mbar_init(fullB + 8 * s, 1); mbar_init(emptyB + 8 * s, 2); }   // emptyB: one arrival per issuer
-    for (int b = 0; b < 2; ++b) { mbar_init(accFull + 8 * b, 2); mbar_init(accEmpty + 8 * b, 4); }
+    // fullA: the 32 lanes of the slot's warp; emptyA / emptyB: one arrival per consumer warpgroup
+    for (int s = 0; s < sa; ++s) { mbar_init(fullA + 8 * s, 32); mbar_init(emptyA + 8 * s, 2); }
+    for (int s = 0; s < sb; ++s) { mbar_init(fullB + 8 * s, 1); mbar_init(emptyB + 8 * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == CH_W_MMA) {   // all 512 TMEM columns: two accumulator buffers of 256 columns (one CTA per SM, no contention)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_misc[0])), "r"(512u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   unsigned bar_gen = 0;
   if (tid == 0 && gbar) bar_gen = ld_acquire_u32(gbar + 1);    // before this launch's first barrier can complete
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
   // Everything above touched no data of an earlier kernel in the stream; from here on we read activations.
   if (flags & 1) asm volatile("griddepcontrol.wait;" ::: "memory");
-  const uint32_t tmem_base = s_misc[0];
   if (dbg_clock && tid == 0) dbg_clock[blockIdx.x * 32 + 1] = clock64();
 
   // pipeline state of this thread's role; persists over items and layers
-  uint32_t a_slot = 0, a_phase = 0, b_slot = 0, b_phase = 0, n_item = 0;
+  uint32_t a_slot = 0, a_phase = 0, b_slot = 0, b_phase = 0;
   uint32_t g_slot = 0;                             // gather producers: row slots the CTA has gone through before the current item
-  uint32_t p_sl = warp >= CH_W_A ? (uint32_t)(warp - CH_W_A) : 0u, p_lapb = 0, p_par = 0;   // gather producers: my next ring slot, global index of slot 0 of its lap, lap parity
+  uint32_t p_sl = (warp >= CH_W_A && warp < CH_W_A + CH_A_WARPS) ? (uint32_t)(warp - CH_W_A) : 0u, p_lapb = 0, p_par = 0;   // gather producers: my next ring slot, global index of slot 0 of its lap, lap parity
 
   for (int L = 0; L < n_layers; ++L) {
     __syncthreads();                                   // every role is done with the previous layer (and with s_ss)
@@ -272,14 +378,13 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
           t_begin = min(z * d_sps, T), t_end = min(t_begin + d_sps, T);                                        \
           (_n = nsub, true))
 
-    const long long _role_t0 = prof ? clock64() : 0;
     if (warp == CH_W_B) {
       // ============================ weight tiles ====================================
       const uint8_t *wtiles = s_desc->wtiles;
       CH_FOR_ITEMS() {
         (void)m;
         for (int t = t_begin; t < t_end; ++t) {
-          { CH_PROF_BEGIN(); mbar_wait_relaxed(emptyB + 8 * b_slot, b_phase ^ 1, 64); CH_PROF_END(pw0); }
+          mbar_wait_relaxed(emptyB + 8 * b_slot, b_phase ^ 1, 64);
           if (elect_one()) {
             const uint32_t fb = fullB + 8 * b_slot;
             if (flags & 0x200) {                      // tuning: no weight loads
@@ -293,104 +398,7 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
           if (++b_slot == (uint32_t)sb) { b_slot = 0; b_phase ^= 1; }
         }
       }
-    } else if (warp == CH_W_MMA || warp == CH_W_MMA + 1) {
-      // ============ MMA issuers: warp CH_W_MMA owns sub-tile 0 of every item, the next warp sub-tile 1 ===============
-      // One issuing thread spends ~64 cycles per tcgen05.mma plus ~400 cycles of barrier-wait / fence / commit per row
-      // slot, more than the 288 cycles of tensor work a 96-channel slot carries; two issuers on disjoint accumulator
-      // columns restore the slack two co-resident CTAs used to give.  Each sub-tile's MMAs are issued by one thread, in
-      // stage order (bit-reproducible accumulation).
-      const int mi = warp - CH_W_MMA;
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(d_nt >> 3) << 17) | ((uint32_t)(CH_M >> 4) << 24);
-      CH_FOR_ITEMS() {
-        (void)m; (void)nti;
-        const uint32_t buf = n_item & 1u;
-        const bool mine = mi < nsub;
-        // Both issuers follow the full protocol of every item, also the one without a sub-tile of its own (single-sub-tile
-        // items): its arrivals on emptyB / accFull may only happen in the phase they belong to, i.e. after the same waits.
-        { CH_PROF_BEGIN(); mbar_wait(accEmpty + 8 * buf, ((n_item >> 1) & 1u) ^ 1u); CH_PROF_END(pw2); }   // the epilogue drained this buffer
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t dcol = tmem_base + buf * 256u + (uint32_t)mi * 128u;
-        // two stages per iteration: the fixed cost of an iteration (waits, proxy fence, election, descriptor set-up) is a
-        // dependent chain of a few hundred cycles; 12 MMAs behind it instead of 6
-        for (int t = t_begin; t < t_end;) {
-          const int nst = min(2, t_end - t);
-          uint32_t sl[2], sph[2], bs[2], bph[2];
-          {
-            uint32_t as_ = a_slot + (uint32_t)mi, ap_ = a_phase, bs_ = b_slot, bp_ = b_phase;
-            if (as_ >= (uint32_t)sa) { as_ -= (uint32_t)sa; ap_ ^= 1u; }
-#pragma unroll
-            for (int jx = 0; jx < 2; ++jx) {
-              sl[jx] = as_; sph[jx] = ap_; bs[jx] = bs_; bph[jx] = bp_;
-              as_ += (uint32_t)nsub; if (as_ >= (uint32_t)sa) { as_ -= (uint32_t)sa; ap_ ^= 1u; }
-              if (++bs_ == (uint32_t)sb) { bs_ = 0; bp_ ^= 1u; }
-            }
-          }
-          if (mine) {
-            {                                         // all barriers of the batch probed together (overlapping round trips)
-              CH_PROF_BEGIN();
-              const bool two = nst == 2;
-              const uint32_t b1 = two ? bs[1] : bs[0], bp1 = two ? bph[1] : bph[0], a1 = two ? sl[1] : sl[0], ap1 = two ? sph[1] : sph[0];
-              for (uint32_t it = 0;; ++it) {
-                const uint32_t ok = mbar_try(fullB + 8 * bs[0], bph[0]) & mbar_try(fullA + 8 * sl[0], sph[0]) &
-                                    mbar_try(fullB + 8 * b1, bp1) & mbar_try(fullA + 8 * a1, ap1);
-                if (ok) break;
-                if (it > (1u << 26)) __trap();
-              }
-              CH_PROF_END(pw1);
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) writes -> UMMA reads
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (flags & 0x4000) {                     // tuning: plain arrivals instead of tcgen05.commit (only without MMAs)
-              if (lane == 0) {
-#pragma unroll
-                for (int jx = 0; jx < 2; ++jx)
-                  if (jx < nst) { mbar_arrive(emptyA + 8 * sl[jx]); mbar_arrive(emptyB + 8 * bs[jx]); }
-              }
-            } else if (elect_one()) {
-#pragma unroll
-              for (int jx = 0; jx < 2; ++jx) {
-                if (jx < nst) {
-                  const uint64_t db = umma_desc(b_ring_k + bs[jx] * (uint32_t)bslot);
-                  const uint64_t da = umma_desc(a_ring_k + sl[jx] * (uint32_t)CH_A_BYTES);
-                  // 128-byte line = [hi ch0-15 | hi ch16-31 | lo ch0-15 | lo ch16-31]; +2 per 32-byte K slice
-#pragma unroll
-                  for (int h = 0; h < 2; ++h) {
-                    if (flags & 0x400) break;         // tuning: no MMAs
-                    umma_bf16(dcol, da + 2 * h, db + 2 * h, idesc, (h == 0 && jx == 0 && t == t_begin) ? 0u : 1u);   // hi * Whi
-                    umma_bf16(dcol, da + 2 * h, db + 2 * h + 4, idesc, 1u);                                          // hi * Wlo
-                    umma_bf16(dcol, da + 2 * h + 4, db + 2 * h, idesc, 1u);                                          // lo * Whi
-                  }
-                  umma_commit(emptyA + 8 * sl[jx]);                         // row slot free when these MMAs retire
-                  umma_commit(emptyB + 8 * bs[jx]);                         // weight slot: one arrival per issuer
-                }
-              }
-            }
-          } else {
-#pragma unroll
-            for (int jx = 0; jx < 2; ++jx) {
-              if (jx < nst) {
-                mbar_wait(fullB + 8 * bs[jx], bph[jx]);                     // stay in step with the slot's phase ...
-                if (lane == 0) mbar_arrive(emptyB + 8 * bs[jx]);            // ... nothing of mine reads this weight tile
-              }
-            }
-          }
-          __syncwarp();
-#pragma unroll
-          for (int jx = 0; jx < 2; ++jx) {
-            if (jx < nst) {
-              a_slot += (uint32_t)nsub;
-              if (a_slot >= (uint32_t)sa) { a_slot -= (uint32_t)sa; a_phase ^= 1u; }
-              if (++b_slot == (uint32_t)sb) { b_slot = 0; b_phase ^= 1; }
-            }
-          }
-          t += nst;
-        }
-        if (mine) { if (elect_one()) umma_commit(accFull + 8 * buf); }
-        else if (lane == 0) mbar_arrive(accFull + 8 * buf);
-        __syncwarp();
-        ++n_item;
-      }
-    } else if (warp >= CH_W_A) {
+    } else if (warp < CH_W_MMA) {
       // ================= gathered A rows: warp w fills every CH_A_WARPS-th row slot, all 128 rows of it ====================
       // 8 lanes cover one 128-byte row line (one L2 line), 4 rows per copy instruction, 32 instructions per slot behind ONE
       // barrier wait and ONE (self-tracking) arrival; the destination carries the 128B swizzle (chunk ^ (row & 7)); a
@@ -409,7 +417,7 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
         (void)nti;
         const uint32_t n_slots = (uint32_t)((t_end - t_begin) * nsub), g_end = g_slot + n_slots;
         auto decode = [&](uint32_t jl_, int &k_, int &cb_, int &s_) {
-          const int st = (int)jl_ / nsub;             // stage-major, sub-tile-minor: the order the issuers consume slots in
+          const int st = (int)jl_ / nsub;             // stage-major, sub-tile-minor: the order the consumers take slots in
           s_ = (int)jl_ - st * nsub;
           const int tt = t_begin + st;
           k_ = tt / nb; cb_ = tt - k_ * nb;
@@ -428,13 +436,8 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
         if (owner && p_lapb + p_sl < g_end) { decode(p_lapb + p_sl - g_slot, k_n, cb_n, s_n); fetch(k_n, s_n, nxt); }
         while (owner && p_lapb + p_sl < g_end) {
           int32_t cur[4];
-          {
-            CH_PROF_BEGIN();
 #pragma unroll
-            for (int i = 0; i < 4; ++i) cur[i] = nxt[i];
-            if (prof) { if (cur[0] + cur[1] + cur[2] + cur[3] == 0x7fffffff) pw2 += 1; }   // force the loads to land here
-            CH_PROF_END(pw1);
-          }
+          for (int i = 0; i < 4; ++i) cur[i] = nxt[i];
           const int cb = cb_n;
           const uint32_t sl = p_sl, par = p_par, jl = p_lapb + p_sl - g_slot;
           // my next slot (same warp, CH_A_WARPS slots on or the next lap)
@@ -444,7 +447,7 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
           const bool first = cb < d_nb0;
           const uint8_t *src = (first ? src0 : src1) + (first ? cb : cb - d_nb0) * 128;
           const uint32_t rb = first ? rb0 : rb1;
-          { CH_PROF_BEGIN(); chain_wait(emptyA + 8 * sl, par ^ 1u, 4 | ((int)jl << 8)); CH_PROF_END(pw0); }
+          chain_wait(emptyA + 8 * sl, par ^ 1u, 4 | ((int)jl << 8));
           const uint32_t a_dst = a_ring_k + sl * (uint32_t)CH_A_BYTES;
           if (!(flags & 0x100)) {                     // tuning: bit 8 = no row copies
 #pragma unroll
@@ -457,8 +460,7 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
                 const int i = g8 * 8 + ii;
                 const uint32_t rr = r8[ii] < 0 ? 0u : (uint32_t)r8[ii];
                 // src-size form (16 or 0 bytes): the copy engine itself writes the zeros of a missing neighbour, so they are
-                // covered by the self-tracking arrival below.  (The ignore-src predicate form produced intermittently stale
-                // rows in the slot that is consumed right after it is filled: profiles/r02_chain_roles.md.)
+                // covered by the self-tracking arrival below (zeros written by any other path would not be).
                 cp_async16(a_dst + (uint32_t)(i >> 1) * 1024u + ((i & 1) ? off_odd : off_even), src + (uint64_t)rr * rb,
                            r8[ii] < 0 ? 0u : 16u);
               }
@@ -468,140 +470,33 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
         }
         g_slot = g_end;
       }
-    } else if (warp < 4) {
-      // ================= epilogue: four warps drain both accumulator buffers in turn ====================
-      // (their own work is ~5% of a layer; the other four warps of the former second group gather rows now)
-      const int q = warp & 3;                         // TMEM lane quarter this warp may access
-      const uint32_t stgw = stg_u32 + (uint32_t)warp * 4096u;
-      const int rsub = lane >> 3, chunk = lane & 7, sw = lane & 7;
-      const uint32_t my_line = stgw + lane * 128;
-      const int d_cout = s_desc->cout, d_cout_pad = s_desc->cout_pad, d_relu = s_desc->relu, d_cmap_cout = s_desc->cmap_cout;
-      const bool has_scale = s_desc->scale != nullptr;
-      const uint8_t *d_res = s_desc->res;
-      uint8_t *d_out_split = s_desc->out_split;
-      float *d_out_f32 = s_desc->out_f32, *d_partial = s_desc->partial;
-      const int32_t *d_row_map = s_desc->out_row_map, *d_cmap = s_desc->cmap;
-      auto lds128 = [](uint32_t a) { uint4 v; asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a)); return v; };
-      auto sts128 = [](uint32_t a, uint4 v) { asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory"); };
+    } else {
+      // ============ consumers: warpgroup g multiplies rows [64g, 64g+64) of every sub-tile of an item, then stores them ========
+      // (chain_item, one instance per N-tile width and sub-tile count: two sub-tiles only with N tiles of at most 128 columns)
+      const int g = (warp - CH_W_MMA) >> 2;
+      const ChainRings R{a_ring_k, b_ring_k, (uint32_t)bslot, (uint32_t)sa, (uint32_t)sb, fullA, emptyA, fullB, emptyB};
+      const uint32_t stgw = stg_u32 + (uint32_t)(warp - CH_W_MMA) * 2048u;
+      const bool no_store = (flags & 0x800) != 0;
+      const int nch = d_nt / 32;
       CH_FOR_ITEMS() {
-        const uint32_t buf = n_item & 1u;
-        { CH_PROF_BEGIN(); mbar_wait_relaxed(accFull + 8 * buf, (n_item >> 1) & 1u, 128); CH_PROF_END(pw0); }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int s = 0; s < nsub; ++s) {
-          const int64_t wrow0 = (int64_t)(m + s) * CH_M + q * 32;        // first global row of this warp
-          const int64_t o = wrow0 + lane;
-          int32_t my_orow = (int32_t)min(o, d_n_out - 1);
-          if (d_row_map && o < d_n_out) my_orow = __ldg(d_row_map + o);
-          // staged tile (32 rows x 128 B, swizzled) -> global, 4 full lines per instruction
-          auto flush_tile = [&](uint8_t *base, int64_t row_bytes, int64_t col_byte, bool mapped) {
-            uint4 v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int r = 4 * i + rsub;
-              v[i] = lds128(stgw + r * 128 + ((chunk ^ (r & 7)) << 4));
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int r = 4 * i + rsub;
-              const int32_t mo = __shfl_sync(0xffffffffu, my_orow, r);
-              const int64_t grow = mapped ? (int64_t)mo : wrow0 + r;
-              if (wrow0 + r < d_n_out && grow >= 0 && !(flags & 0x800))
-                *reinterpret_cast<uint4 *>(base + grow * row_bytes + col_byte + chunk * 16) = v[i];
-            }
-          };
-          for (int cbo = 0; cbo < d_nt / 32; ++cbo) {
-            float y[32];
-            {
-              uint32_t v0[16], v1[16];
-              const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * 256u + (uint32_t)s * 128u + cbo * 32;
-              tmem_ld16(taddr, v0);
-              tmem_ld16(taddr + 16, v1);
-              asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-              for (int jj = 0; jj < 16; ++jj) { y[jj] = __uint_as_float(v0[jj]); y[16 + jj] = __uint_as_float(v1[jj]); }
-            }
-            const int c0 = nti * d_nt + cbo * 32;             // first output channel of this 32-block
-            if (d_nsplit > 1) {                               // raw partial sums; the reduce phase applies the epilogue
-#pragma unroll
-              for (int g = 0; g < 8; ++g)
-                sts128(my_line + ((g ^ sw) << 4), make_uint4(__float_as_uint(y[4 * g]), __float_as_uint(y[4 * g + 1]),
-                                                             __float_as_uint(y[4 * g + 2]), __float_as_uint(y[4 * g + 3])));
-              __syncwarp();
-              flush_tile(reinterpret_cast<uint8_t *>(d_partial + (int64_t)z * d_n_out * d_cout_pad), (int64_t)d_cout_pad * 4,
-                         (int64_t)c0 * 4, false);
-              __syncwarp();
-              continue;
-            }
-            if (c0 >= d_cout) continue;                       // warp-uniform (padding columns)
-            int oc0 = c0, out_c = d_cout, kch = 0;
-            if (d_cmap) {                                     // dense transposed conv: this column block belongs to child kch
-              kch = c0 / d_cmap_cout;
-              oc0 = c0 - kch * d_cmap_cout;
-              out_c = d_cmap_cout;
-              my_orow = (o < d_n_out) ? __ldg(d_cmap + (int64_t)kch * d_n_out + o) : -1;
-            }
-            if (has_scale) {
-#pragma unroll
-              for (int jj = 0; jj < 32; ++jj) y[jj] = fmaf(y[jj], s_ss[oc0 + jj], s_ss[CH_SS_FLOATS + oc0 + jj]);
-            }
-            if (d_res) {                                      // residual tile: coalesced load -> staging -> own row
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int r = 4 * i + rsub;
-                uint4 v = make_uint4(0, 0, 0, 0);
-                if (wrow0 + r < d_n_out)
-                  v = __ldcg(reinterpret_cast<const uint4 *>(d_res + (wrow0 + r) * (int64_t)d_cout * 4 + (c0 >> 5) * 128 + chunk * 16));
-                sts128(stgw + r * 128 + ((chunk ^ (r & 7)) << 4), v);
-              }
-              __syncwarp();
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                const uint4 hq = lds128(my_line + ((g ^ sw) << 4)), lq = lds128(my_line + (((4 + g) ^ sw) << 4));
-                const __nv_bfloat16 *hh = reinterpret_cast<const __nv_bfloat16 *>(&hq);
-                const __nv_bfloat16 *ll = reinterpret_cast<const __nv_bfloat16 *>(&lq);
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) y[g * 8 + jj] += join_bf16(hh[jj], ll[jj]);
-              }
-              __syncwarp();
-            }
-            if (d_relu) {
-#pragma unroll
-              for (int jj = 0; jj < 32; ++jj) y[jj] = fmaxf(y[jj], 0.f);
-            }
-            if (d_out_split) {
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                __align__(16) __nv_bfloat16 hh[8], ll[8];
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) split_bf16(y[g * 8 + jj], hh[jj], ll[jj]);
-                sts128(my_line + ((g ^ sw) << 4), *reinterpret_cast<const uint4 *>(hh));
-                sts128(my_line + (((4 + g) ^ sw) << 4), *reinterpret_cast<const uint4 *>(ll));
-              }
-              __syncwarp();
-              flush_tile(d_out_split, (int64_t)out_c * 4, (int64_t)(oc0 >> 5) * 128, d_cmap != nullptr);
-              __syncwarp();
-            }
-            if (d_out_f32) {
-#pragma unroll
-              for (int g = 0; g < 8; ++g)
-                sts128(my_line + ((g ^ sw) << 4), make_uint4(__float_as_uint(y[4 * g]), __float_as_uint(y[4 * g + 1]),
-                                                             __float_as_uint(y[4 * g + 2]), __float_as_uint(y[4 * g + 3])));
-              __syncwarp();
-              flush_tile(reinterpret_cast<uint8_t *>(d_out_f32), (int64_t)out_c * 4, (int64_t)oc0 * 4,
-                         d_row_map != nullptr || d_cmap != nullptr);
-              __syncwarp();
-            }
+#define CH_ITEM(n, s)                                                                                                  \
+          case n: chain_item<n, s>(R, *s_desc, s_ss, stgw, no_store, a_slot, a_phase, b_slot, b_phase, t_begin, t_end, z, nti, \
+                                   m, g, warp, lane); break;
+        if (nsub == 2) {
+          switch (nch) {
+            CH_ITEM(1, 2) CH_ITEM(2, 2)
+            default: __trap();                        // osb_conv_desc_fill pairs sub-tiles only for N tiles <= CH_MAX_PAIR_NT
+          }
+        } else {
+          switch (nch) {
+            CH_ITEM(1, 1) CH_ITEM(2, 1) CH_ITEM(3, 1) CH_ITEM(4, 1)
+            default: __trap();                        // osb_conv_desc_fill plans N tiles of at most 128 columns
           }
         }
-        // this warp's TMEM reads of the buffer are complete (tcgen05.wait::ld above): hand it back to the MMA warps
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(accEmpty + 8 * buf);
-        ++n_item;
+#undef CH_ITEM
       }
     }
 #undef CH_FOR_ITEMS
-    if (prof) pt += clock64() - _role_t0;
 
     if (d_nsplit > 1) {
       // ---- split-K: every partial is in global memory after this barrier; reduce + epilogue by all threads of the grid
@@ -652,15 +547,6 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
   }
 
   if (dbg_clock && tid == 0) dbg_clock[blockIdx.x * 32 + 2] = clock64();
-  if (dbg_clock && lane == 0 && (warp == CH_W_B || warp == CH_W_MMA || warp == CH_W_MMA + 1 || warp == CH_W_A || warp == 0)) {
-    // rows of 4: [wait kind 0, wait kind 1, wait kind 2, role loop total]; B producer 4.., issuer0 8.., issuer1 12.., A producer 16.., epilogue 20..
-    const int base = warp == CH_W_B ? 4 : warp == CH_W_MMA ? 8 : warp == CH_W_MMA + 1 ? 12 : warp == CH_W_A ? 16 : 20;
-    long long *o = dbg_clock + blockIdx.x * 32 + base;
-    o[0] = pw0; o[1] = pw1; o[2] = pw2; o[3] = pt;
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == CH_W_MMA) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
 }
 
 // ------------------------------------------------------------ tile-major, pre-swizzled weight packing
@@ -693,8 +579,12 @@ __global__ void k_pack_weight_tiles(const float *__restrict__ w, int K, int cin,
 namespace osb { bool conv_tc_tuning(const char *name, int64_t v); }
 using namespace osb;
 
-static inline int chain_cout_pad(int cout) { return cout <= 256 ? (cout + 15) / 16 * 16 : (cout + 255) / 256 * 256; }
-static inline int chain_nt(int cout) { const int cp = chain_cout_pad(cout); return cp <= 256 ? cp : 256; }
+// Tile shapes keep a consumer thread at most 64 fp32 accumulators ((64 rows x N columns) / 128 threads per sub-tile), which
+// fit its registers beside the kernel's persistent state with no spill: N tiles of at most 128 columns, and two sub-tiles
+// per item only for N tiles of at most 64 columns (CH_MAX_PAIR_NT).  Wider outputs are padded to whole 128-column tiles.
+static inline int chain_cout_pad(int cout) { return cout <= 128 ? (cout + 15) / 16 * 16 : (cout + 127) / 128 * 128; }
+static inline int chain_nt(int cout) { const int cp = chain_cout_pad(cout); return cp <= 128 ? cp : 128; }
+constexpr int CH_MAX_PAIR_NT = 64;
 
 extern "C" {
 
@@ -707,7 +597,7 @@ int osb_conv_pack_weight_tiles(const float *w, int32_t K, int32_t cin, int32_t c
   OSB_CHECK(K >= 1 && cin % 32 == 0 && cin > 0 && cout > 0, "osb_conv_pack_weight_tiles: cin (%d) must be a multiple of 32", cin);
   const int cp = chain_cout_pad(cout), nt = chain_nt(cout);
   const int64_t total = (int64_t)K * cp * cin;
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(total, 256), 148 * 32);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(total, 256), 132 * 32);
   k_pack_weight_tiles<<<grid, 256, 0, stream>>>(w, K, cin, cout, cp, nt, transpose_w, (uint8_t *)wtiles);
   OSB_LAUNCH_CHECK();
   return 0;
@@ -718,16 +608,17 @@ int osb_conv_pack_weight_tiles(const float *w, int32_t K, int32_t cin, int32_t c
 // busy CTA), so a small cost model may RAISE the factor when it predicts a clear gain (it never lowers it: for the smallest
 // levels the measured optimum is the base rule):
 //   main loop   per CTA (pairs of units x ~0.75 us + single units x ~0.6 us) x stages per split; an item is two row-adjacent
-//               units when the N tile is <= 128 wide (two issuers run them side by side); 1.6x for 256-wide N tiles
+//               units when the N tile is <= CH_MAX_PAIR_NT wide; 1.6x for wider N tiles
 //   split cost  ~10 us (grid barrier, partial tiles out, reduce pass) + the partials written and read once at ~5 TB/s (L2)
-// Constants fitted on the per-layer times of the bench scene (scripts/layer_times.py with OSB_CHAIN_MAX_TILES=0).
+// The constants are rough per-stage costs of the bench scene's layers; the rules above (never lower than the base rule,
+// a clear predicted gain to raise it) keep a mis-fitted constant from doing harm.
 static int chain_nsplit(int64_t n_out, int K, int cin, int cout, int grid_ctas, int force, int nsub_knob) {
   const int cp = chain_cout_pad(cout), nt = chain_nt(cout);
   const int64_t tiles = ceil_div(n_out, CH_M) * (cp / nt);
   const int T = K * (cin / 32);
   const int cap = std::max(1, std::min(32, T));
   if (force > 0) return std::min(force, cap);
-  const bool pairs = nt <= 128 && nsub_knob >= 2;
+  const bool pairs = nt <= CH_MAX_PAIR_NT && nsub_knob >= 2;
   const int base = (int)std::max<int64_t>(1, std::min<int64_t>(grid_ctas / tiles, cap));
   auto cost = [&](int ns, bool &ok) {
     const int sps = (T + ns - 1) / ns;
@@ -757,8 +648,7 @@ static int g_chain_nsub = 2;             // tuning: 1 = never pair sub-tiles
 static int g_chain_grid = 0;             // tuning: CTAs per launch (0 = one per SM)
 static int g_chain_sa = 0, g_chain_sb = 0;   // tuning: ring depths (0 = as many row slots as fit / 3 or 2 weight slots)
 static long long *g_chain_dbg_clock = nullptr;
-static int g_chain_dbg_skip = 0;         // tuning: bit0 no row copies, bit1 no weight loads, bit2 no MMAs, bit3 no stores,
-                                         // bit5 no tcgen05 fence, bit6 plain arrivals for commits, bit8 legacy (consumer-side) completion
+static int g_chain_dbg_skip = 0;         // tuning: bit0 no row copies, bit1 no weight loads, bit3 no stores
 
 int osb_tuning_set(const char *name, int64_t value) {
   const std::string n(name ? name : "");
@@ -778,10 +668,10 @@ int osb_tuning_set(const char *name, int64_t value) {
 }
 
 int osb_conv_chain_grid(void) {
-  if (g_chain_grid > 0) return g_chain_grid;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
+  // the grid barrier needs every CTA resident at once: one CTA per SM at most
+  return g_chain_grid > 0 ? std::min(g_chain_grid, sms) : sms;
 }
 
 size_t osb_conv_chain_workspace_bytes(int64_t n_out, int32_t K, int32_t cin, int32_t cout) {
@@ -813,7 +703,7 @@ int osb_conv_desc_fill(void *desc_host, const void *src0, int32_t c0, const void
   d.out_row_map = out_row_map; d.cmap = cmap; d.n_out = n_out; d.K = K; d.nb0 = c0 / 32; d.nb1 = c1 / 32;
   d.cout = cout; d.cout_pad = chain_cout_pad(cout); d.nt = chain_nt(cout); d.n_ntiles = d.cout_pad / d.nt;
   d.relu = relu; d.cmap_cout = cmap_cout; d.m_tiles = (int)ceil_div(n_out, CH_M);
-  d.nsub_max = (d.nt <= 128 && g_chain_nsub >= 2) ? 2 : 1;
+  d.nsub_max = (d.nt <= CH_MAX_PAIR_NT && g_chain_nsub >= 2) ? 2 : 1;
   d.barrier_before = barrier_before ? 1 : 0;
   d.nsplit = cmap ? 1 : chain_nsplit(n_out, K, cin, cout, osb_conv_chain_grid(), g_chain_force_split, g_chain_nsub);
   const int T = K * (cin / 32);
@@ -861,9 +751,10 @@ int osb_conv_chain_launch(const void *descs_host, int32_t n_layers, void *grid_b
     int sa = (227 * 1024 - fixed - sb * bslot) / CH_A_BYTES;
     if (g_chain_sa > 0) sa = std::min(sa, g_chain_sa);
     sa = std::min(sa, CH_MAX_SA);
-    // An EVEN ring: with two sub-tiles per stage every row slot (and its two barriers) then belongs to one issuer for good.
-    // With an odd ring the slots alternate between the issuers from lap to lap; a two-pipeline variant of this kernel produced
-    // intermittently stale rows on hardware exactly then (and never with even rings): profiles/r02_chain_roles.md.
+    // An EVEN ring: the two row slots of a paired stage then never straddle the end of the ring, and these are the ring
+    // shapes tests/test_chain_protocol_model.py proves safe and live.  At least four slots: a consumer warpgroup holds the
+    // row slots of two paired stages at once (it releases a stage's slots once the next stage's wgmmas are issued and the
+    // previous group has retired).
     sa &= ~1;
     OSB_CHECK(sa >= 4, "osb_conv_chain_launch: shared memory does not hold four row slots");
     const size_t smem_bytes = (size_t)sa * CH_A_BYTES + (size_t)sb * bslot + fixed;

@@ -257,7 +257,7 @@ template <int CIN>
 static int launch_fwd_thin(const float *in, const int32_t *nbr, int64_t n_out, int K, const float *w, float *out, cudaStream_t stream) {
   const size_t smem = (size_t)K * CIN * THIN_COUT * sizeof(float);
   OSB_SMEM_ATTR_ONCE(k_conv_fwd_thin<CIN>, 96 * 1024);
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n_out, 8), 148 * 8);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n_out, 8), 132 * 8);
   k_conv_fwd_thin<CIN><<<grid, 256, smem, stream>>>(in, nbr, n_out, K, w, out);
   OSB_LAUNCH_CHECK();
   return 0;
@@ -265,7 +265,7 @@ static int launch_fwd_thin(const float *in, const int32_t *nbr, int64_t n_out, i
 
 template <int CIN>
 static int launch_wgrad_thin(const float *in, const int32_t *nbr, int64_t n_out, int K, const float *gout, float *gw, cudaStream_t stream) {
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n_out, THIN_WG_ROWS), 148 * 4);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n_out, THIN_WG_ROWS), 132 * 4);
   k_conv_wgrad_thin<CIN><<<grid, THIN_WG_WARPS * 32, 0, stream>>>(in, nbr, n_out, K, gout, gw);
   OSB_LAUNCH_CHECK();
   return 0;
@@ -330,7 +330,7 @@ int osb_gather_rows_f32(const float *in, const int32_t *idx, int64_t n_out, int3
   if (n_out == 0) return 0;
   OSB_CHECK(n_out > 0 && c > 0 && in && idx && out, "osb_gather_rows_f32: bad arguments (n_out %lld, c %d)", (long long)n_out, c);
   const int64_t total = n_out * c;
-  unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(total, 256), 148 * 16);
+  unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(total, 256), 132 * 16);
   k_gather_rows_f32<<<blocks, 256, 0, stream>>>(in, idx, n_out, c, out);
   OSB_LAUNCH_CHECK();
   return 0;

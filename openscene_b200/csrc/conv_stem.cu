@@ -133,7 +133,7 @@ int osb_conv_stem_fused(const float *in, int32_t cin, const int32_t *coords, int
   if (stem_check(cin, cout, ks, out_split, scale, shift, n, &smem)) return 1;
   OSB_CHECK(slots != nullptr && cap > 0 && (cap & (cap - 1)) == 0, "osb_conv_stem_fused: bad hash table");
   OSB_SMEM_ATTR_ONCE(k_conv_stem<StemHashLookup>, 200 * 1024);
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, STEM_WARPS), 148 * 3);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, STEM_WARPS), 132 * 3);
   const StemHashLookup lk{(const HashSlot *)slots, (uint64_t)cap - 1};
   k_conv_stem<StemHashLookup><<<grid, STEM_WARPS * 32, smem, stream>>>(in, cin, (const int4 *)coords, n, lk, ks, step, w, cout, scale,
                                                                        shift, relu, (uint8_t *)out_split, out_f32);
@@ -157,7 +157,7 @@ int osb_conv_stem_fused_grid(const float *in, int32_t cin, const int32_t *coords
   lk.g.bitmap = reinterpret_cast<const unsigned long long *>(grid_);
   lk.g.first_row = reinterpret_cast<const int32_t *>(reinterpret_cast<const unsigned long long *>(grid_) + words);
   lk.g.nbits = nbits; lk.g.log2_ts = log2_ts; lk.g.n_batch = n_batch;
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, STEM_WARPS), 148 * 3);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, STEM_WARPS), 132 * 3);
   k_conv_stem<StemGridLookup><<<grid, STEM_WARPS * 32, smem, stream>>>(in, cin, (const int4 *)coords, n, lk, ks, step, w, cout, scale,
                                                                        shift, relu, (uint8_t *)out_split, out_f32);
   OSB_LAUNCH_CHECK();

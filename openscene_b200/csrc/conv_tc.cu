@@ -1,4 +1,4 @@
-// Sparse convolution on 5th-gen tensor cores: TMA gather4 -> shared memory -> tcgen05.mma -> TMEM.
+// Sparse convolution on tensor cores: gathered rows -> shared memory -> wgmma -> register accumulators.
 //
 //   out[o,:] = epilogue( sum_k  in[nbr[k][o], :] @ W[k] )         (output-stationary, no atomics)
 //
@@ -7,45 +7,44 @@
 // folded in (mink_unet.py:50,114,147; BasicBlock).
 //
 // Numerics: fp32 operands are carried as split bf16 pairs (v = hi + lo) and every product is
-// evaluated as hi*Whi + hi*Wlo + lo*Whi on kind::f16 (bf16) MMAs with fp32 accumulation in TMEM:
+// evaluated as hi*Whi + hi*Wlo + lo*Whi on bf16 wgmma with fp32 accumulation:
 // ~2^-16 relative operand error, i.e. fp32-grade results at 1.5x the tensor time of one TF32 pass.
 //
 // One CTA = 128 output rows x NT output channels.  A pipeline stage holds one (offset k, 32-channel
-// block) pair: A = 128 gathered rows x 128 B (TMA tile::gather4, 128B swizzle, missing neighbours are
-// out-of-bounds rows -> hardware zero fill, no L2 traffic), B = NT weight rows x 128 B.
-// Warp roles: 0 = TMA producer of the weight tiles, 1 = TMEM alloc + MMA issuer, 2..5 = producers of
-// the gathered A rows (32 rows per warp) during the main loop, then the epilogue (TMEM -> registers ->
-// affine/residual/ReLU -> split-bf16 or fp32 rows).
-// Three A paths are kept selectable (osb_debug_set_tc), measured on B200 on the level-0 96->96 3^3 layer:
+// block) pair: A = 128 gathered rows x 128 B (128B swizzle; a missing neighbour is a zero-filled row),
+// B = NT weight rows x 128 B (TMA tile load).
+// Warpgroup 0 produces: warp w gathers rows [32w, 32w+32), warp 0 also loads the weight tiles.  Warpgroups
+// 1 and 2 each multiply 64 rows of the tile (M64 x NT x K16 wgmma, accumulators in registers), then run the
+// epilogue on them (affine/residual/ReLU -> split-bf16 or fp32 rows, through a swizzled staging tile).
+// Two A paths are kept selectable (osb_tuning_set "tc_a_path"):
 //   2 (default) cp.async.cg 16 B x 8 lanes per row, swizzled by hand, completion through
 //               cp.async.mbarrier.arrive.noinc on the stage's full barrier;
-//   1           TMA tile::gather4 (4 rows x 128 B per instruction): the TMA unit spends ~20-25 cycles per
-//               gather4 instruction regardless of bytes (~23 B/clk/SM), which bounds the whole kernel;
-//   0           one TMA row load per row (cross-check path).
+//   0           one TMA row load per row (cross-check path; a missing row is an out-of-bounds row: zero fill).
 #include "tc_ptx.cuh"
 #include <algorithm>
 #include <string>
 
 namespace osb {
 
-constexpr int TC_M = 128;          // rows per CTA (UMMA M)
+constexpr int TC_M = 128;          // rows per CTA
 constexpr int TC_MAXK = 32;        // kernel offsets handled by this kernel (27, 8, 1)
-constexpr int TC_THREADS = 192;
+constexpr int TC_THREADS = 384;    // producer warpgroup + two consumer warpgroups
 constexpr int TC_A_BYTES = TC_M * 128;
+constexpr int TC_STG_BYTES = 8 * 2048;   // epilogue staging: 8 consumer warps x (16 rows x 128 B)
 
 struct ConvTcParams {
   const int32_t *nbr;
   int64_t n_out;
   int K, nb0, nb1;
   int n_src0, n_src1;
-  int cout, cout_pad, nt, stages, tmem_cols;
+  int cout, cout_pad, nt, stages;
   const float *scale, *shift;
   const uint8_t *res;
   int relu;
   uint8_t *out_split;
   float *out_f32;
   const int32_t *out_row_map;
-  int use_gather4;
+  int use_cpasync;       // A path: 1 = cp.async gathers, 0 = TMA row loads
   int nsplit;            // > 1: blockIdx.z handles a contiguous chunk of the (offset, channel-block) stage sequence
   float *partial;        // [nsplit][n_out][cout_pad] raw accumulators (nsplit > 1)
   const uint8_t *src0_ptr, *src1_ptr;   // raw bases (L2 prefetch of a later tile's own rows)
@@ -59,47 +58,45 @@ struct ConvTcParams {
 };
 
 // ------------------------------------------------------------------------------------ the kernel
-__global__ void __launch_bounds__(TC_THREADS)
+template <int NCH>   // NT = 32 * NCH output channels per CTA
+__global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
           const __grid_constant__ CUtensorMap tmB, const ConvTcParams p) {
+  constexpr int NT = 32 * NCH;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int stage_bytes = TC_A_BYTES + p.nt * 128;
-  uint8_t *aux = smem + p.stages * stage_bytes;
+  const int stage_bytes = TC_A_BYTES + NT * 128;
+  const uint32_t stg_base = smem_u32(smem + p.stages * stage_bytes);
+  uint8_t *aux = smem + p.stages * stage_bytes + TC_STG_BYTES;
   int32_t *s_nbr = reinterpret_cast<int32_t *>(aux);                        // [K][128]
   float *s_scale = reinterpret_cast<float *>(aux + (p.lazy_idx ? 0 : p.K * TC_M * 4));   // [nt]
   float *s_shift = s_scale + 256;                                           // [nt]
-  uint64_t *bars = reinterpret_cast<uint64_t *>(s_shift + 256);             // full[8], empty[8], accum
-  uint32_t *s_misc = reinterpret_cast<uint32_t *>(bars + 17);               // [0] tmem base, [1] kmask
+  uint64_t *bars = reinterpret_cast<uint64_t *>(s_shift + 256);             // full[8], empty[8]
+  uint32_t *s_misc = reinterpret_cast<uint32_t *>(bars + 16);               // [0] kmask
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (p.pdl) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the next kernel may start its prologue
-  if (p.dbg_clock && tid == 64) { p.dbg_clock[blockIdx.x * 8 + 0] = clock64(); unsigned sm; asm("mov.u32 %0, %%smid;" : "=r"(sm)); p.dbg_clock[blockIdx.x * 8 + 7] = sm; }
+  if (p.dbg_clock && tid == 0) { p.dbg_clock[blockIdx.x * 8 + 0] = clock64(); unsigned sm; asm("mov.u32 %0, %%smid;" : "=r"(sm)); p.dbg_clock[blockIdx.x * 8 + 7] = sm; }
   const int64_t row0 = (int64_t)blockIdx.x * TC_M;
-  const int n0 = blockIdx.y * p.nt;
-  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 8), accum_bar = smem_u32(bars + 16);
+  const int n0 = blockIdx.y * NT;
+  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 8);
 
-  if (tid == 32 * 2) {
+  if (tid == 32) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA0) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA1) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
   if (tid == 0) {
-    const uint32_t full_count = p.use_gather4 == 2 ? 1 + 128 : 1;     // B producer (+ 128 cp.async A producers)
-    for (int s = 0; s < p.stages; ++s) { mbar_init(full0 + 8 * s, full_count); mbar_init(empty0 + 8 * s, 1); }
-    mbar_init(accum_bar, 1);
-    s_misc[1] = 0;
+    const uint32_t full_count = p.use_cpasync ? 1 + 128 : 1;     // B producer (+ 128 cp.async A producers)
+    // empty: one arrival per consumer warpgroup
+    for (int s = 0; s < p.stages; ++s) { mbar_init(full0 + 8 * s, full_count); mbar_init(empty0 + 8 * s, 2); }
+    s_misc[0] = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {   // TMEM allocation (whole warp), result written to smem
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_misc[0])),
-                 "r"((uint32_t)p.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  __syncthreads();   // s_misc[1] = 0 visible before the atomics below
+  __syncthreads();   // s_misc[0] = 0 visible before the atomics below
 
   // ---- prologue: neighbour rows of this tile -> smem, bit mask of offsets that touch the tile.
-  // All loads of a thread are issued before any is consumed (22 = ceil(32*128/192) independent loads).
+  // All loads of a thread are issued before any is consumed (11 = ceil(32*128/384) independent loads).
   if (!p.lazy_idx) {
     constexpr int PRO = (TC_MAXK * TC_M + TC_THREADS - 1) / TC_THREADS;
     int32_t idx[PRO];
@@ -123,23 +120,20 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       }
     }
     mymask = __reduce_or_sync(0xffffffffu, mymask);
-    if (lane == 0 && mymask) atomicOr(&s_misc[1], mymask);
+    if (lane == 0 && mymask) atomicOr(&s_misc[0], mymask);
   }
-  for (int n = tid; n < p.nt; n += TC_THREADS) {
+  for (int n = tid; n < NT; n += TC_THREADS) {
     const int c = n0 + n;
     const int cc = p.cmap ? c % p.cmap_cout : c;
     s_scale[n] = (p.scale && c < p.cout) ? __ldg(p.scale + cc) : 1.f;
     s_shift[n] = (p.shift && c < p.cout) ? __ldg(p.shift + cc) : 0.f;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
   // Everything above touched only launch-invariant data (kernel map, BN constants).  The activations, the residual
   // and the shared split workspace belong to the previous kernel in the stream: wait for it to finish and flush.
   if (p.pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
-  const uint32_t tmem_base = s_misc[0];
-  const uint32_t kmask = (p.dbg_skip & 4) ? 0u : (p.lazy_idx ? (p.K >= 32 ? 0xffffffffu : ((1u << p.K) - 1u)) : s_misc[1]);
-  if (p.dbg_clock && tid == 64) p.dbg_clock[blockIdx.x * 8 + 1] = clock64();
+  const uint32_t kmask = (p.dbg_skip & 4) ? 0u : (p.lazy_idx ? (p.K >= 32 ? 0xffffffffu : ((1u << p.K) - 1u)) : s_misc[0]);
+  if (p.dbg_clock && tid == 0) p.dbg_clock[blockIdx.x * 8 + 1] = clock64();
   const int nb = p.nb0 + p.nb1;
   // stage sequence of this tile = (valid offsets in ascending k) x (channel blocks); split mode takes a chunk
   const int n_stage_all = __popc(kmask) * nb;
@@ -149,11 +143,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     t_begin = min((int)blockIdx.z * per, n_stage_all);
     t_end = min(t_begin + per, n_stage_all);
   }
-  const bool have_work = t_end > t_begin;
 
-  if (warp == 0) {
-    // ============================ TMA producer: weight tiles =========================
-    if (p.pf_dist > 0 && blockIdx.y == 0 && blockIdx.z == 0 && elect_one()) {
+  if (warp < 4) {
+    // ============ producers: warp w gathers rows [32w, 32w+32) of every stage; warp 0 also loads the weight tiles ============
+    const int w = warp;
+    if (warp == 0 && p.pf_dist > 0 && blockIdx.y == 0 && blockIdx.z == 0 && elect_one()) {
       // Stride-1 convolutions read mostly the rows around their own tile (Morton order): pull the rows of the
       // tile that will run ~one wave later into L2 now, so its gathers do not wait on compulsory DRAM misses.
       const int64_t r0 = ((int64_t)blockIdx.x + p.pf_dist) * TC_M;
@@ -167,97 +161,55 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
         }
       }
     }
+    __syncwarp();
+    const int j = lane & 7, q = lane >> 3;
     int s = 0;
     uint32_t phase = 0;
     int t = 0;
+    // lazy mode: this thread's 8 row indices of offset k come straight from the kernel map (L2), prefetched one
+    // offset ahead so that the load latency hides behind the copies of the current offset
+    auto fetch = [&](int k, int32_t (&r)[8]) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int64_t o = row0 + w * 32 + 4 * i + q;
+        r[i] = (o < p.n_out) ? (p.nbr ? __ldg(p.nbr + (int64_t)k * p.n_out + o) : (int32_t)o) : -1;
+      }
+    };
+    int32_t rnext[8];
+    if (p.lazy_idx && kmask) fetch(__ffs(kmask) - 1, rnext);
     for (uint32_t km = kmask; km; km &= km - 1) {
       const int k = __ffs(km) - 1;
+      int32_t ridx[8];
+      if (p.lazy_idx) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) ridx[i] = rnext[i];
+        const uint32_t rest = km & (km - 1);
+        if (rest) fetch(__ffs(rest) - 1, rnext);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) ridx[i] = s_nbr[k * TC_M + w * 32 + 4 * i + q];
+      }
       for (int cb = 0; cb < nb; ++cb, ++t) {
         if (t < t_begin || t >= t_end) continue;
         mbar_wait(empty0 + 8 * s, phase ^ 1);
-        if (elect_one()) {
-          const uint32_t fb = full0 + 8 * s;
-          uint32_t bytes = (uint32_t)stage_bytes;        // A (4 warps x 8 gathers) + B bytes of this stage
-          if ((p.dbg_skip & 1) || p.use_gather4 == 2) bytes -= TC_A_BYTES;
-          if (p.dbg_skip & 2) bytes -= p.nt * 128;
+        const uint32_t fb = full0 + 8 * s;
+        const uint32_t a_base = smem_u32(smem + s * stage_bytes);
+        if (warp == 0 && elect_one()) {
+          uint32_t bytes = (uint32_t)stage_bytes;        // A (TMA row path) + B bytes of this stage
+          if ((p.dbg_skip & 1) || p.use_cpasync) bytes -= TC_A_BYTES;
+          if (p.dbg_skip & 2) bytes -= NT * 128;
           mbar_expect_tx(fb, bytes);
-          if (!(p.dbg_skip & 2))
-            tma_load_2d(smem_u32(smem + s * stage_bytes) + TC_A_BYTES, &tmB, fb, cb * 64, k * p.cout_pad + n0);
+          if (!(p.dbg_skip & 2)) tma_load_2d(a_base + TC_A_BYTES, &tmB, fb, cb * 64, k * p.cout_pad + n0);
         }
         __syncwarp();
-        if (++s == p.stages) { s = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ===================================
-    // instruction descriptor: D=f32, A=B=bf16, K-major both, N = nt, M = 128
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.nt >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-    int s = 0;
-    uint32_t phase = 0, acc = 0;
-    for (int t = t_begin; t < t_end; ++t) {
-      {
-        mbar_wait(full0 + 8 * s, phase);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) writes -> UMMA reads
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (elect_one()) {
-          const uint32_t a_addr = smem_u32(smem + s * stage_bytes);
-          const uint64_t da = umma_desc(a_addr), db = umma_desc(a_addr + TC_A_BYTES);
-          // 128-byte line = [hi ch0-15 | hi ch16-31 | lo ch0-15 | lo ch16-31]; +2 per 32-byte K slice
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            umma_bf16(tmem_base, da + 2 * h, db + 2 * h, idesc, (h == 0) ? acc : 1u);   // hi * Whi
-            umma_bf16(tmem_base, da + 2 * h, db + 2 * h + 4, idesc, 1);     // hi * Wlo
-            umma_bf16(tmem_base, da + 2 * h + 4, db + 2 * h, idesc, 1);     // lo * Whi
-          }
-          umma_commit(empty0 + 8 * s);      // frees the stage when these MMAs retire
-        }
-        acc = 1;
-        __syncwarp();
-        if (++s == p.stages) { s = 0; phase ^= 1; }
-      }
-    }
-    if (elect_one()) umma_commit(accum_bar);
-    __syncwarp();
-  } else {
-    // ================= A producers (32 rows per warp), then epilogue ====================
-    if (p.use_gather4 == 2) {
-      // cp.async producers: 8 lanes cover one 128-byte row line (one L2 line per 8 lanes), 4 rows per warp
-      // instruction, 8 instructions per stage; destination carries the 128B swizzle (chunk ^ (row & 7)).
-      const int w = warp - 2, j = lane & 7, q = lane >> 3;
-      int s = 0;
-      uint32_t phase = 0;
-      int t = 0;
-      // lazy mode: this thread's 8 row indices of offset k come straight from the kernel map (L2), prefetched one
-      // offset ahead so that the load latency hides behind the copies of the current offset
-      auto fetch = [&](int k, int32_t (&r)[8]) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int64_t o = row0 + w * 32 + 4 * i + q;
-          r[i] = (o < p.n_out) ? (p.nbr ? __ldg(p.nbr + (int64_t)k * p.n_out + o) : (int32_t)o) : -1;
-        }
-      };
-      int32_t rnext[8];
-      if (p.lazy_idx && kmask) fetch(__ffs(kmask) - 1, rnext);
-      for (uint32_t km = kmask; km; km &= km - 1) {
-        const int k = __ffs(km) - 1;
-        int32_t ridx[8];
-        if (p.lazy_idx) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) ridx[i] = rnext[i];
-          const uint32_t rest = km & (km - 1);
-          if (rest) fetch(__ffs(rest) - 1, rnext);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) ridx[i] = s_nbr[k * TC_M + w * 32 + 4 * i + q];
-        }
-        for (int cb = 0; cb < nb; ++cb, ++t) {
-          if (t < t_begin || t >= t_end) continue;
-          mbar_wait(empty0 + 8 * s, phase ^ 1);
-          const bool first = cb < p.nb0;
+        const bool first = cb < p.nb0;
+        if (p.use_cpasync) {
+          // 8 lanes cover one 128-byte row line (one L2 line per 8 lanes), 4 rows per warp instruction, 8 instructions
+          // per stage; the destination carries the 128B swizzle (chunk ^ (row & 7)).
           const uint8_t *src = first ? p.src0_ptr : p.src1_ptr;
           const int64_t row_bytes = (int64_t)(first ? p.nb0 : p.nb1) * 128;
           const int col_byte = (first ? cb : cb - p.nb0) * 128 + j * 16;
-          const uint32_t a_dst = smem_u32(smem + s * stage_bytes) + (w * 32 + q) * 128;
+          const uint32_t a_dst = a_base + (w * 32 + q) * 128;
           if (!(p.dbg_skip & 1)) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
@@ -267,183 +219,117 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
               cp_async16(a_dst + i * 512 + ((j ^ m7) << 4), sp, valid ? 16u : 0u);      // size 0 -> zero fill
             }
           }
-          cp_async_arrive_noinc(full0 + 8 * s);
-          if (++s == p.stages) { s = 0; phase ^= 1; }
-        }
-      }
-    } else {
-      const int w = warp - 2;                     // rows [32w, 32w+32) of the tile
-      int s = 0;
-      uint32_t phase = 0;
-      int t = 0;
-      for (uint32_t km = kmask; km; km &= km - 1) {
-        const int k = __ffs(km) - 1;
-        const int32_t *rows = s_nbr + k * TC_M + w * 32;
-        for (int cb = 0; cb < nb; ++cb, ++t) {
-          if (t < t_begin || t >= t_end) continue;
-          mbar_wait(empty0 + 8 * s, phase ^ 1);
-          if (elect_one() && !(p.dbg_skip & 1)) {
-            const uint32_t a_dst = smem_u32(smem + s * stage_bytes) + w * 4096;
-            const uint32_t fb = full0 + 8 * s;
-            const bool first = cb < p.nb0;
-            const CUtensorMap *tm = first ? &tmA0 : &tmA1;
-            const int col = (first ? cb : cb - p.nb0) * 64;
-            const int oob = first ? p.n_src0 : p.n_src1;       // one past the last row: hardware zero fill
+          cp_async_arrive_noinc(fb);
+        } else if (!(p.dbg_skip & 1)) {
+          // one TMA row load per row; a missing row reads one past the last row: hardware zero fill
+          const CUtensorMap *tm = first ? &tmA0 : &tmA1;
+          const int col = (first ? cb : cb - p.nb0) * 64;
+          const int oob = first ? p.n_src0 : p.n_src1;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int4 r4 = *reinterpret_cast<const int4 *>(rows + 4 * j);
-              const int r0 = r4.x >= 0 ? r4.x : oob, r1 = r4.y >= 0 ? r4.y : oob;
-              const int r2 = r4.z >= 0 ? r4.z : oob, r3 = r4.w >= 0 ? r4.w : oob;
-              if (p.use_gather4) {
-                tma_gather4(a_dst + j * 512, tm, fb, col, r0, r1, r2, r3);
-              } else {   // same tensor map, one row per copy (debug / cross-check path)
-                tma_load_2d(a_dst + j * 512, tm, fb, col, r0);
-                tma_load_2d(a_dst + j * 512 + 128, tm, fb, col, r1);
-                tma_load_2d(a_dst + j * 512 + 256, tm, fb, col, r2);
-                tma_load_2d(a_dst + j * 512 + 384, tm, fb, col, r3);
-              }
-            }
+          for (int rr = 0; rr < 32; ++rr) {
+            const int r = __shfl_sync(0xffffffffu, ridx[rr >> 2], 8 * (rr & 3));   // row rr = 4i + q is held by lanes 8q..8q+7
+            if (lane == 0) tma_load_2d(a_base + (w * 32 + rr) * 128, tm, fb, col, r >= 0 ? r : oob);
           }
-          __syncwarp();
-          if (++s == p.stages) { s = 0; phase ^= 1; }
         }
+        if (++s == p.stages) { s = 0; phase ^= 1; }
       }
     }
-    if (p.dbg_clock && tid == 64) p.dbg_clock[blockIdx.x * 8 + 2] = clock64();     // A producers done issuing
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    const int m = q * 32 + lane;
-    const int64_t o = row0 + m;
-    if (have_work) {
-      mbar_wait(accum_bar, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    if (p.dbg_clock && tid == 0) p.dbg_clock[blockIdx.x * 8 + 2] = clock64();     // producers done issuing
+  } else {
+    // ============ consumers: warpgroup g multiplies tile rows [64g, 64g+64), then runs their epilogue ============
+    const int g = (warp >> 2) - 1;
+    float acc[16 * NCH];
+#pragma unroll
+    for (int i = 0; i < 16 * NCH; ++i) acc[i] = 0.f;
+    int s = 0, s_prev = -1;
+    uint32_t phase = 0;
+    for (int t = t_begin; t < t_end; ++t) {
+      mbar_wait(full0 + 8 * s, phase);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) writes -> wgmma reads
+      const uint32_t a_addr = smem_u32(smem + s * stage_bytes);
+      wgmma_fence();
+      wg_split_mma<NCH>(acc, gmma_desc(a_addr + g * 64 * 128), gmma_desc(a_addr + TC_A_BYTES));
+      wgmma_commit();
+      wgmma_wait<1>();                                               // the previous stage's wgmmas have retired: free it
+      if (s_prev >= 0 && (tid & 127) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(empty0 + 8 * s_prev) : "memory");
+      s_prev = s;
+      if (++s == p.stages) { s = 0; phase ^= 1; }
     }
-    if (p.dbg_clock && tid == 64) p.dbg_clock[blockIdx.x * 8 + 3] = clock64();     // accumulator ready
-    // Rows of this warp: tile rows [32q, 32q+32).  Global traffic goes through a 4 KB shared-memory staging
-    // tile per warp (pipeline stage 0 is idle by now) in the 128B-swizzled layout, so that every global
-    // load / store instruction moves 4 full 128-byte lines (lane -> row 4i + lane/8, 16-byte chunk lane%8)
-    // instead of 32 half-sectors.
+    wgmma_wait<0>();
+    wgmma_hold(acc);
+    if (p.dbg_clock && tid == 128) p.dbg_clock[blockIdx.x * 8 + 3] = clock64();     // accumulator ready
+    // Rows of this warp: tile rows [64g + 16(warp%4), +16).  Global traffic goes through a 2 KB staging tile per warp in
+    // the 128B-swizzled layout, so that every global load / store instruction moves 4 full 128-byte lines.
     const bool no_store = (p.dbg_skip & 8) != 0;
-    const uint32_t stg = smem_u32(smem) + q * 4096;
-    const int64_t wrow0 = row0 + q * 32;                         // first global row of this warp
-    const int rsub = lane >> 3, chunk = lane & 7;
-    int32_t my_orow = (int32_t)min(o, p.n_out - 1);
-    if (p.out_row_map && o < p.n_out) my_orow = __ldg(p.out_row_map + o);
-    auto lds128 = [](uint32_t a) { uint4 v; asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a)); return v; };
-    auto sts128 = [](uint32_t a, uint4 v) { asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory"); };
-    const uint32_t my_line = stg + lane * 128;
-    const int sw = lane & 7;
-    // staged tile -> global: dst_row(r) gives the destination row index of tile row r (or -1)
-    auto flush_tile = [&](uint8_t *base, int64_t row_bytes, int64_t col_byte, bool mapped) {
-      uint4 v[8];
+    const uint32_t stg = stg_base + (uint32_t)(warp - 4) * 2048u;
+    const int64_t wrow0 = row0 + 64 * g + 16 * (warp & 3);         // first global row of this warp
+    const int cq = 2 * (lane & 3);
+    auto plain_row = [&](int r) -> int64_t { return (!no_store && wrow0 + r < p.n_out) ? wrow0 + r : -1; };
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {                 // all shared loads first, then all global stores
-        const int r = 4 * i + rsub;
-        v[i] = lds128(stg + r * 128 + ((chunk ^ (r & 7)) << 4));
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int r = 4 * i + rsub;
-        const int32_t mo = __shfl_sync(0xffffffffu, my_orow, r);
-        const int64_t grow = mapped ? (int64_t)mo : wrow0 + r;
-        if (wrow0 + r < p.n_out && !no_store && grow >= 0)
-          *reinterpret_cast<uint4 *>(base + grow * row_bytes + col_byte + chunk * 16) = v[i];
-      }
-    };
-    for (int cbo = 0; cbo < p.nt / 32; ++cbo) {
-      float y[32];
-      if (have_work) {
-        uint32_t v0[16], v1[16];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + cbo * 32;
-        tmem_ld16(taddr, v0);
-        tmem_ld16(taddr + 16, v1);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { y[j] = __uint_as_float(v0[j]); y[16 + j] = __uint_as_float(v1[j]); }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) y[j] = 0.f;
-      }
+    for (int cbo = 0; cbo < NCH; ++cbo) {
+      float *y = acc + 16 * cbo;
       const int c0 = n0 + cbo * 32;              // first output channel of this 32-block
       if (p.nsplit > 1) {                        // raw partial sums; k_conv_finish reduces + applies the epilogue
-#pragma unroll
-        for (int g = 0; g < 8; ++g)
-          sts128(my_line + ((g ^ sw) << 4), make_uint4(__float_as_uint(y[4 * g]), __float_as_uint(y[4 * g + 1]),
-                                                       __float_as_uint(y[4 * g + 2]), __float_as_uint(y[4 * g + 3])));
+        frag_stage_f32(stg, y, lane);
         __syncwarp();
-        flush_tile(reinterpret_cast<uint8_t *>(p.partial + (int64_t)blockIdx.z * p.n_out * p.cout_pad), (int64_t)p.cout_pad * 4,
-                   (int64_t)c0 * 4, false);
+        stage_flush(stg, reinterpret_cast<uint8_t *>(p.partial + (int64_t)blockIdx.z * p.n_out * p.cout_pad), (int64_t)p.cout_pad * 4,
+                    (int64_t)c0 * 4, lane, plain_row);
         __syncwarp();
         continue;
       }
       if (c0 >= p.cout) continue;               // warp-uniform
       if (p.scale != nullptr) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) y[j] = fmaf(y[j], s_scale[cbo * 32 + j], s_shift[cbo * 32 + j]);
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int col = cbo * 32 + 8 * i + cq + (e & 1);
+            y[4 * i + e] = fmaf(y[4 * i + e], s_scale[col], s_shift[col]);
+          }
       }
-      if (p.res) {                               // residual tile: coalesced load -> smem -> own row
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int r = 4 * i + rsub;
-          uint4 v = make_uint4(0, 0, 0, 0);
-          if (wrow0 + r < p.n_out)
-            v = __ldg(reinterpret_cast<const uint4 *>(p.res + (wrow0 + r) * (int64_t)p.cout * 4 + (c0 >> 5) * 128 + chunk * 16));
-          sts128(stg + r * 128 + ((chunk ^ (r & 7)) << 4), v);
-        }
+      if (p.res) {                               // residual tile: coalesced load -> staging -> own fragment
+        stage_load(stg, p.res, wrow0, p.n_out, (int64_t)p.cout * 4, (int64_t)(c0 >> 5) * 128, lane);
         __syncwarp();
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const uint4 hq = lds128(my_line + ((g ^ sw) << 4)), lq = lds128(my_line + (((4 + g) ^ sw) << 4));
-          const __nv_bfloat16 *hh = reinterpret_cast<const __nv_bfloat16 *>(&hq);
-          const __nv_bfloat16 *ll = reinterpret_cast<const __nv_bfloat16 *>(&lq);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) y[g * 8 + j] += join_bf16(hh[j], ll[j]);
-        }
+        frag_add_split(stg, y, lane);
         __syncwarp();
       }
       if (p.relu) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) y[j] = fmaxf(y[j], 0.f);
+        for (int e = 0; e < 16; ++e) y[e] = fmaxf(y[e], 0.f);
       }
       int oc0 = c0;                                  // first output channel of this block in the destination row
       int out_c = p.cout;                            // channels per destination row
-      if (p.cmap) {                                  // dense transposed conv: this column block belongs to child k
-        const int kch = c0 / p.cmap_cout;
+      int kch = 0;
+      if (p.cmap) {                                  // dense transposed conv: this column block belongs to child kch
+        kch = c0 / p.cmap_cout;
         oc0 = c0 - kch * p.cmap_cout;
         out_c = p.cmap_cout;
-        my_orow = (o < p.n_out) ? __ldg(p.cmap + (int64_t)kch * p.n_out + o) : -1;
       }
+      auto cmap_row = [&](int r) -> int64_t {
+        return (!no_store && wrow0 + r < p.n_out) ? (int64_t)__ldg(p.cmap + (int64_t)kch * p.n_out + wrow0 + r) : -1;
+      };
       if (p.out_split) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          __align__(16) __nv_bfloat16 hh[8], ll[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) split_bf16(y[g * 8 + j], hh[j], ll[j]);
-          sts128(my_line + ((g ^ sw) << 4), *reinterpret_cast<const uint4 *>(hh));
-          sts128(my_line + (((4 + g) ^ sw) << 4), *reinterpret_cast<const uint4 *>(ll));
-        }
+        frag_stage_split(stg, y, lane);
         __syncwarp();
-        flush_tile(p.out_split, (int64_t)out_c * 4, (int64_t)(oc0 >> 5) * 128, p.cmap != nullptr);
+        if (p.cmap) stage_flush(stg, p.out_split, (int64_t)out_c * 4, (int64_t)(oc0 >> 5) * 128, lane, cmap_row);
+        else stage_flush(stg, p.out_split, (int64_t)out_c * 4, (int64_t)(oc0 >> 5) * 128, lane, plain_row);
         __syncwarp();
       }
       if (p.out_f32) {
-#pragma unroll
-        for (int g = 0; g < 8; ++g)
-          sts128(my_line + ((g ^ sw) << 4), make_uint4(__float_as_uint(y[4 * g]), __float_as_uint(y[4 * g + 1]),
-                                                       __float_as_uint(y[4 * g + 2]), __float_as_uint(y[4 * g + 3])));
+        frag_stage_f32(stg, y, lane);
         __syncwarp();
-        flush_tile(reinterpret_cast<uint8_t *>(p.out_f32), (int64_t)out_c * 4, (int64_t)oc0 * 4, p.out_row_map != nullptr || p.cmap != nullptr);
+        uint8_t *base = reinterpret_cast<uint8_t *>(p.out_f32);
+        if (p.cmap) stage_flush(stg, base, (int64_t)out_c * 4, (int64_t)oc0 * 4, lane, cmap_row);
+        else if (p.out_row_map)
+          stage_flush(stg, base, (int64_t)out_c * 4, (int64_t)oc0 * 4, lane, [&](int r) -> int64_t {
+            return (!no_store && wrow0 + r < p.n_out) ? (int64_t)__ldg(p.out_row_map + wrow0 + r) : -1;
+          });
+        else stage_flush(stg, base, (int64_t)out_c * 4, (int64_t)oc0 * 4, lane, plain_row);
         __syncwarp();
       }
     }
   }
-
-  if (p.dbg_clock && tid == 64) p.dbg_clock[blockIdx.x * 8 + 4] = clock64();       // epilogue stores issued
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (p.dbg_clock && tid == 64) p.dbg_clock[blockIdx.x * 8 + 5] = clock64();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols));
-  }
+  if (p.dbg_clock && tid == 128) p.dbg_clock[blockIdx.x * 8 + 4] = clock64();     // epilogue stores issued
 }
 
 // ------------------------------------------------------------------ split-mode finish kernel
@@ -549,23 +435,23 @@ static int make_tmap(CUtensorMap *tm, const void *base, uint64_t cols_elems, uin
   return make_tmap_2b(tm, base, cols_elems, rows, box_rows, 0);
 }
 
-static int g_tc_use_gather4 = 2;            // A operand path: 2 = cp.async (default), 1 = TMA gather4, 0 = TMA row loads
-static int g_tc_smem_budget = 112 * 1024;   // per CTA -> two CTAs per SM
+static int g_tc_a_path = 2;                 // A operand path: 2 = cp.async (default), 0 = TMA row loads
+static int g_tc_smem_budget = 227 * 1024;   // per CTA: the register file holds one 384-thread CTA per SM
 static int g_tc_dbg_skip = 0;
 static int g_tc_force_split = 0;            // 0 = heuristic, >0 = forced nsplit (1 disables)
-static int g_tc_target_ctas = 148;          // split small launches until ~one CTA per SM (sweep: profiles/r01_tune_conv.md)
+static int g_tc_target_ctas = 132;          // split small launches until ~one CTA per SM (H100 SXM: 132 SMs)
 static int g_tc_pf_dist = 0;
 static int g_tc_small_nt = 0;              // > 0: N tile used when the launch has few row tiles (tuning)
 static int g_tc_small_rows = 5120;
 static int g_tc_min_stages = 3;
-static int g_tc_lazy = 1;                  // cp.async path: per-offset index fetch instead of the smem index prologue            // fewest stages accepted for the multi-CTA-per-SM configuration
+static int g_tc_lazy = 1;                  // cp.async path: per-offset index fetch instead of the smem index prologue
 static long long *g_tc_dbg_clock = nullptr;
 
 // knobs of this kernel behind osb_tuning_set (conv_chain.cu); returns false for names it does not own
 bool conv_tc_tuning(const char *name, int64_t v) {
   const std::string n(name);
-  if (n == "tc_a_path") g_tc_use_gather4 = (int)v;            // 2 = cp.async (default), 1 = TMA gather4, 0 = TMA row loads
-  else if (n == "tc_smem_budget") g_tc_smem_budget = (int)v;  // per CTA; 112 KB -> two CTAs per SM
+  if (n == "tc_a_path") g_tc_a_path = (int)v;                 // 2 = cp.async (default), 0 = TMA row loads
+  else if (n == "tc_smem_budget") g_tc_smem_budget = (int)v;  // per CTA
   else if (n == "tc_dbg_skip") g_tc_dbg_skip = (int)v;
   else if (n == "tc_force_split") g_tc_force_split = (int)v;
   else if (n == "tc_target_ctas") g_tc_target_ctas = (int)v;
@@ -614,7 +500,7 @@ int osb_conv_pack_weights(const float *w, int32_t K, int32_t cin, int32_t cout, 
   OSB_CHECK(K >= 1 && cin % 32 == 0 && cin > 0 && cout > 0, "osb_conv_pack_weights: cin (%d) must be a multiple of 32", cin);
   const int cp = cout_pad_of(cout);
   const int64_t total = (int64_t)K * cp * cin;
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(total, 256), 148 * 32);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(total, 256), 132 * 32);
   k_pack_weights<<<grid, 256, 0, stream>>>(w, K, cin, cout, cp, transpose_w, (uint8_t *)wpack);
   OSB_LAUNCH_CHECK();
   return 0;
@@ -664,20 +550,19 @@ static int conv_fwd_tc_impl(const void *src0, int32_t c0, int64_t n_src0, const 
   const int cp = cout_pad_of(cout);
   ConvTcParams p{};
   p.nt = choose_nt(n_out, cp);
+  OSB_CHECK(g_tc_a_path == 2 || g_tc_a_path == 0, "osb_conv_fwd_tc: A path %d does not exist (2 = cp.async, 0 = TMA rows)", g_tc_a_path);
   const int stage_bytes = TC_A_BYTES + p.nt * 128;
-  // lazy index fetch pays off on multi-wave launches (level 0: every tile touches all K offsets, the smem prologue is pure
-  // set-up cost: 325 -> 298 us); on single-wave levels skipping empty (tile, offset) stages wins (59 vs 68 us at level 1)
-  const int lazy = (g_tc_use_gather4 == 2 && g_tc_lazy == 1 && ceil_div(n_out, TC_M) >= 592) || g_tc_lazy == 2 ? 1 : 0;
-  const int aux_bytes = (lazy ? 0 : K * TC_M * 4) + 2 * 256 * 4 + 17 * 8 + 64;
+  // lazy index fetch pays off on multi-wave launches (every tile touches all K offsets, the smem prologue is pure set-up
+  // cost); on single-wave levels skipping empty (tile, offset) stages wins
+  const int lazy = (g_tc_a_path == 2 && g_tc_lazy == 1 && ceil_div(n_out, TC_M) >= 4 * 132) || g_tc_lazy == 2 ? 1 : 0;
+  const int aux_bytes = TC_STG_BYTES + (lazy ? 0 : K * TC_M * 4) + 2 * 256 * 4 + 16 * 8 + 64;
   const int seq = K * (cin / 32);                                         // stages one tile runs through (upper bound)
-  int stages = (g_tc_smem_budget - 1024 - aux_bytes) / stage_bytes;      // two CTAs per SM if that leaves >= 3 stages ...
-  if (stages < g_tc_min_stages && !(stages == 2 && seq <= 4))            // ... or the whole sequence is that short anyway
+  int stages = (g_tc_smem_budget - 1024 - aux_bytes) / stage_bytes;      // what the budget holds (default: the whole SM) ...
+  if (stages < g_tc_min_stages && !(stages == 2 && seq <= 4))            // ... unless that is too few for a longer sequence
     stages = (226 * 1024 - 1024 - aux_bytes) / stage_bytes;
   stages = std::max(2, std::min(8, std::min(stages, std::max(2, seq))));
   const size_t smem_bytes = (size_t)stages * stage_bytes + aux_bytes + 1024;
   OSB_CHECK(smem_bytes <= 227 * 1024, "osb_conv_fwd_tc: tile does not fit in shared memory");
-  int tmem_cols = 32;
-  while (tmem_cols < p.nt) tmem_cols <<= 1;
 
   CUtensorMap tmA0, tmA1, tmB;
   if (make_tmap(&tmA0, src0, 2ull * c0, (uint64_t)n_src0, 1)) return 1;
@@ -687,10 +572,10 @@ static int conv_fwd_tc_impl(const void *src0, int32_t c0, int64_t n_src0, const 
 
   p.nbr = nbr; p.n_out = n_out; p.K = K; p.nb0 = c0 / 32; p.nb1 = c1 / 32;
   p.n_src0 = (int)n_src0; p.n_src1 = (int)n_src1;
-  p.cout = cout; p.cout_pad = cp; p.stages = stages; p.tmem_cols = tmem_cols;
+  p.cout = cout; p.cout_pad = cp; p.stages = stages;
   p.scale = scale; p.shift = shift; p.res = (const uint8_t *)res; p.relu = relu;
   p.out_split = (uint8_t *)out_split; p.out_f32 = out_f32; p.out_row_map = out_row_map;
-  p.use_gather4 = g_tc_use_gather4;
+  p.use_cpasync = g_tc_a_path == 2 ? 1 : 0;
   p.dbg_skip = g_tc_dbg_skip;
   p.pdl = (flags & 1) ? 1 : 0;
   p.lazy_idx = lazy;
@@ -707,7 +592,6 @@ static int conv_fwd_tc_impl(const void *src0, int32_t c0, int64_t n_src0, const 
     p.partial = (float *)ws;
   }
 
-  OSB_SMEM_ATTR_ONCE(k_conv_tc, 227 * 1024);
   dim3 grid((unsigned)ceil_div(n_out, TC_M), (unsigned)(cp / p.nt), (unsigned)p.nsplit);
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -715,11 +599,20 @@ static int conv_fwd_tc_impl(const void *src0, int32_t c0, int64_t n_src0, const 
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
   cfg.attrs = attr; cfg.numAttrs = p.pdl ? 1 : 0;
-  OSB_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc, tmA0, tmA1, tmB, p));
+  switch (p.nt / 32) {
+#define OSB_TC_CASE(n)                                                 \
+    case n:                                                            \
+      OSB_SMEM_ATTR_ONCE(k_conv_tc<n>, 227 * 1024);                    \
+      OSB_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<n>, tmA0, tmA1, tmB, p)); \
+      break;
+    OSB_TC_CASE(1) OSB_TC_CASE(2) OSB_TC_CASE(3) OSB_TC_CASE(4) OSB_TC_CASE(5) OSB_TC_CASE(6) OSB_TC_CASE(7) OSB_TC_CASE(8)
+#undef OSB_TC_CASE
+    default: OSB_CHECK(false, "osb_conv_fwd_tc: N tile %d not supported", p.nt);
+  }
   OSB_LAUNCH_CHECK();
   if (p.nsplit > 1) {
     const int64_t total = n_out * (cout / 8);
-    const unsigned fgrid = (unsigned)std::min<int64_t>(ceil_div(total, 256), 148 * 8);
+    const unsigned fgrid = (unsigned)std::min<int64_t>(ceil_div(total, 256), 132 * 8);
     cudaLaunchConfig_t fcfg{};
     fcfg.gridDim = dim3(fgrid); fcfg.blockDim = dim3(256); fcfg.dynamicSmemBytes = 0; fcfg.stream = stream;
     fcfg.attrs = attr; fcfg.numAttrs = p.pdl ? 1 : 0;

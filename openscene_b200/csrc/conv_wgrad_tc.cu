@@ -1,15 +1,16 @@
-// Weight gradient of the sparse convolution on 5th-gen tensor cores (run/distill.py:333, `loss.backward()` through
+// Weight gradient of the sparse convolution on tensor cores (wgmma) (run/distill.py:333, `loss.backward()` through
 // every MinkowskiConvolution / MinkowskiConvolutionTranspose of models/mink_unet.py):
 //
 //   gW[k][ci][co] = sum_{o : nbr[k][o] >= 0}  x[nbr[k][o], ci] * gout[o, co]
 //
 // The reduction runs over ROWS, the dimension along which the split-bf16 activations are NOT contiguous: both operands
-// are therefore MN-major UMMA operands.  A 128-byte line of a split row, [hi x32 | lo x32] of one 32-channel block, is 64
+// are therefore MN-major wgmma operands.  A 128-byte line of a split row, [hi x32 | lo x32] of one 32-channel block, is 64
 // consecutive "MN" elements; 8 consecutive rows form the 1024-byte 128B-swizzle atom (physically the same shared-memory
-// image the forward kernel gathers, only read with the transpose bits of the instruction descriptor set).  One MMA
-// (M128 x N<=256 x K16) multiplies 16 rows of two input-channel blocks with 16 rows of up to four output-channel blocks; its
-// fp32 result tile holds, per (block, block) pair, the four products hi*hi, hi*lo, lo*hi, lo*lo, which the reduce kernel
-// adds up (the full (hi+lo)(hi+lo) product: slightly MORE accurate than the three-term forward).
+// image the forward kernel gathers, only read with the transpose bits of the instruction set).  Two warpgroups, one per
+// input-channel block, multiply 16 rows of their block with 16 rows of up to four output-channel blocks per K step
+// (M64 x N64 x K16 each); the fp32 result tile (128 x N<=256) holds, per (block, block) pair, the four products hi*hi, hi*lo,
+// lo*hi, lo*lo, which the reduce kernel adds up (the full (hi+lo)(hi+lo) product: slightly MORE accurate than the
+// three-term forward).
 //
 // Work unit = (offset k, pair of input blocks, group of <= 4 output blocks, range of output rows); one CTA per unit writes
 // its raw 128 x N accumulator to a partial buffer, a second kernel sums quadrants and row ranges in a fixed order: no
@@ -19,7 +20,7 @@
 
 namespace osb {
 
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = 384;             // warpgroup 0: row gathers + gout TMA; warpgroups 1, 2: wgmma + epilogue
 constexpr int WG_ROWS = 128;                 // rows (the MMA K dimension) per pipeline stage
 constexpr int WG_TILE = WG_ROWS * 128;       // one (128 rows x one 32-channel block) tile: 16 KB
 constexpr int WG_STAGES = 2;
@@ -35,19 +36,13 @@ struct WgradParams {
   float *partial;              // [units][128][256] raw accumulators
 };
 
-// MN-major, 128-byte swizzle: 8 K-rows = one 1024-byte atom (SBO), 64-element MN chunks LBO bytes apart
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__global__ void __launch_bounds__(WG_THREADS)
+__global__ void __launch_bounds__(WG_THREADS, 1)
 k_conv_wgrad_tc(const __grid_constant__ CUtensorMap tmG, const WgradParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + WG_STAGES * WG_STAGE_BYTES);    // fullA[2], fullB[2], empty[2], accum
-  uint32_t *s_misc = reinterpret_cast<uint32_t *>(bars + 8);
+  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + WG_STAGES * WG_STAGE_BYTES);    // fullA[2], fullB[2], empty[2]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t fullA = smem_u32(bars), fullB = smem_u32(bars + 2), empty0 = smem_u32(bars + 4), accum_bar = smem_u32(bars + 6);
+  const uint32_t fullA = smem_u32(bars), fullB = smem_u32(bars + 2), empty0 = smem_u32(bars + 4);
 
   // unit -> (k, mt, nt, rs)
   int u = blockIdx.x;
@@ -61,62 +56,17 @@ k_conv_wgrad_tc(const __grid_constant__ CUtensorMap tmG, const WgradParams p) {
   const int n_stage = (int)((r_end - r_begin + WG_ROWS - 1) / WG_ROWS);
 
   if (tid == 0) {
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(fullA + 8 * s, 128); mbar_init(fullB + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-    mbar_init(accum_bar, 1);
+    // fullA: the 128 gathering threads; empty: one arrival per consumer warpgroup
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(fullA + 8 * s, 128); mbar_init(fullB + 8 * s, 1); mbar_init(empty0 + 8 * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (tid == 64) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_misc[0])), "r"(256u));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  if (tid == 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = s_misc[0];
 
-  if (warp == 0) {
-    // ============ gout tiles by TMA: rows [r, r+128) x one 32-channel block each (rows past n_out: zero fill) ============
-    int s = 0; uint32_t phase = 0;
-    for (int t = 0; t < n_stage; ++t) {
-      mbar_wait(empty0 + 8 * s, phase ^ 1);
-      if (elect_one()) {
-        const uint32_t fb = fullB + 8 * s;
-        mbar_expect_tx(fb, (uint32_t)(n_ob * WG_TILE));
-        const int row = (int)(r_begin + (int64_t)t * WG_ROWS);
-        for (int b = 0; b < n_ob; ++b)
-          tma_load_2d(smem_u32(smem + s * WG_STAGE_BYTES + (2 + b) * WG_TILE), &tmG, fb, (ob0 + b) * 64, row);
-      }
-      __syncwarp();
-      if (++s == WG_STAGES) { s = 0; phase ^= 1; }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ===================================
-    // D = f32, A = B = bf16, both operands MN-major (bits 15, 16), N = 64 per output block, M = 128
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)((n_ob * 64) >> 3) << 17) |
-                           ((uint32_t)(128 >> 4) << 24);
-    int s = 0; uint32_t phase = 0;
-    for (int t = 0; t < n_stage; ++t) {
-      mbar_wait(fullB + 8 * s, phase);
-      mbar_wait(fullA + 8 * s, phase);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint32_t base = smem_u32(smem + s * WG_STAGE_BYTES);
-        const uint64_t da = umma_desc_mn(base, WG_TILE), db = umma_desc_mn(base + 2 * WG_TILE, WG_TILE);
-#pragma unroll
-        for (int ks = 0; ks < WG_ROWS / 16; ++ks)          // 16 rows = two 1024-byte atoms per MMA
-          umma_bf16(tmem_base, da + (uint64_t)(ks * 128), db + (uint64_t)(ks * 128), idesc, (t == 0 && ks == 0) ? 0u : 1u);
-        umma_commit(empty0 + 8 * s);
-      }
-      __syncwarp();
-      if (++s == WG_STAGES) { s = 0; phase ^= 1; }
-    }
-    if (elect_one()) umma_commit(accum_bar);
-    __syncwarp();
-  } else {
-    // ============ gathered x rows (32 rows per warp and stage, as in the forward kernels), then the epilogue ============
-    const int w = warp - 2, j = lane & 7, q = lane >> 3;
+  if (warp < 4) {
+    // ===== gathered x rows (32 rows per warp and stage, as in the forward kernels); warp 0 also loads the gout tiles =====
+    // gout tiles by TMA: rows [r, r+128) x one 32-channel block each (rows past n_out: zero fill)
+    const int w = warp, j = lane & 7, q = lane >> 3;
     const int64_t row_bytes = (int64_t)p.nbi * 128;
     int s = 0; uint32_t phase = 0;
     for (int t = 0; t < n_stage; ++t) {
@@ -127,6 +77,14 @@ k_conv_wgrad_tc(const __grid_constant__ CUtensorMap tmG, const WgradParams p) {
         ridx[i] = (o < r_end) ? (p.nbr ? __ldg(p.nbr + (int64_t)k * p.n_out + o) : (int32_t)o) : -1;
       }
       mbar_wait(empty0 + 8 * s, phase ^ 1);
+      if (warp == 0 && elect_one()) {
+        const uint32_t fb = fullB + 8 * s;
+        mbar_expect_tx(fb, (uint32_t)(n_ob * WG_TILE));
+        const int row = (int)(r_begin + (int64_t)t * WG_ROWS);
+        for (int b = 0; b < n_ob; ++b)
+          tma_load_2d(smem_u32(smem + s * WG_STAGE_BYTES + (2 + b) * WG_TILE), &tmG, fb, (ob0 + b) * 64, row);
+      }
+      __syncwarp();
       for (int b = 0; b < 2; ++b) {
         const uint32_t a_dst = smem_u32(smem + s * WG_STAGE_BYTES + b * WG_TILE) + (w * 32 + q) * 128;
         const bool have = b < n_ib;                      // a missing second block is multiplied as zeros (rows 64..127 of D unused)
@@ -141,42 +99,50 @@ k_conv_wgrad_tc(const __grid_constant__ CUtensorMap tmG, const WgradParams p) {
       cp_async_arrive_noinc(fullA + 8 * s);
       if (++s == WG_STAGES) { s = 0; phase ^= 1; }
     }
-    // ---- epilogue: raw accumulator (128 x 64*n_ob fp32) -> partial[unit], full-line coalesced through a staging tile
-    const int qq = warp & 3;                             // TMEM lane quarter
-    mbar_wait(accum_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t stg = smem_u32(smem) + (uint32_t)(warp - 2) * 4096u;
-    const int rsub = lane >> 3, chunk = lane & 7, sw = lane & 7;
-    const uint32_t my_line = stg + lane * 128;
-    float *dst = p.partial + (int64_t)blockIdx.x * 128 * 256;
-    for (int cb = 0; cb < n_ob * 2; ++cb) {
-      uint32_t v0[16], v1[16];
-      const uint32_t taddr = tmem_base + ((uint32_t)(qq * 32) << 16) + cb * 32;
-      tmem_ld16(taddr, v0);
-      tmem_ld16(taddr + 16, v1);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  } else {
+    // ===== wgmma: warpgroup g (1, 2) owns input block ib0 + g - 1 = rows [64(g-1), 64g) of the 128 x N accumulator =====
+    const int g = (warp >> 2) - 1;
+    const bool active = g < n_ib;
+    float acc[4 * 32];
 #pragma unroll
-      for (int g = 0; g < 4; ++g)
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(my_line + ((g ^ sw) << 4)), "r"(v0[4 * g]), "r"(v0[4 * g + 1]),
-                     "r"(v0[4 * g + 2]), "r"(v0[4 * g + 3]) : "memory");
+    for (int i = 0; i < 4 * 32; ++i) acc[i] = 0.f;
+    int s = 0; uint32_t phase = 0;
+    for (int t = 0; t < n_stage; ++t) {
+      mbar_wait(fullB + 8 * s, phase);
+      mbar_wait(fullA + 8 * s, phase);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) writes -> wgmma reads
+      if (active) {
+        const uint32_t base = smem_u32(smem + s * WG_STAGE_BYTES);
+        const uint64_t da = gmma_desc_mn(base + g * WG_TILE, WG_TILE);
+        wgmma_fence();
 #pragma unroll
-      for (int g = 0; g < 4; ++g)
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(my_line + (((4 + g) ^ sw) << 4)), "r"(v1[4 * g]), "r"(v1[4 * g + 1]),
-                     "r"(v1[4 * g + 2]), "r"(v1[4 * g + 3]) : "memory");
-      __syncwarp();
+        for (int ks = 0; ks < WG_ROWS / 16; ++ks)          // 16 rows = two 1024-byte atoms per K step
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int r = 4 * i + rsub;
-        uint4 v;
-        asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(stg + r * 128 + ((chunk ^ (r & 7)) << 4)));
-        *reinterpret_cast<uint4 *>(dst + (int64_t)(qq * 32 + r) * 256 + cb * 32 + chunk * 4) = v;
+          for (int b = 0; b < 4; ++b)
+            if (b < n_ob)
+              wgmma_n64_bf16<1, 1>(acc + 32 * b, da + (uint64_t)(ks * 128), gmma_desc_mn(base + (2 + b) * WG_TILE, WG_TILE) + (uint64_t)(ks * 128), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_hold(acc);
       }
-      __syncwarp();
+      if ((tid & 127) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(empty0 + 8 * s) : "memory");
+      if (++s == WG_STAGES) { s = 0; phase ^= 1; }
+    }
+    // ---- epilogue: raw accumulator rows of this warp -> partial[unit] (rows and columns the reduce kernel reads)
+    if (active) {
+      float *dst = p.partial + (int64_t)blockIdx.x * 128 * 256;
+      const int r = 64 * g + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+      for (int b = 0; b < 4; ++b)
+        if (b < n_ob)
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              *reinterpret_cast<float2 *>(dst + (int64_t)(r + 8 * h) * 256 + 64 * b + 8 * i + cq) =
+                  make_float2(acc[32 * b + 4 * i + 2 * h], acc[32 * b + 4 * i + 2 * h + 1]);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u));
 }
 
 // gw[k][ci][co] = sum over row ranges and over the four (hi|lo) x (hi|lo) quadrants of the unit's accumulator
@@ -208,7 +174,7 @@ static void wgrad_plan(int64_t n_out, int K, int cin, int cout, int *n_mt, int *
   *n_nt = (cout / 32 + 3) / 4;
   const int64_t base = (int64_t)K * *n_mt * *n_nt;
   const int64_t chunks = ceil_div(n_out, WG_ROWS);
-  int64_t rs = std::max<int64_t>(1, (2 * 148 + base - 1) / base);           // about two CTAs' worth of units per SM ...
+  int64_t rs = std::max<int64_t>(1, (2 * 132 + base - 1) / base);           // about two CTAs' worth of units per SM ...
   rs = std::min(rs, std::max<int64_t>(1, chunks / 4));                      // ... but at least 4 stages per unit
   *rows_per_rs = ceil_div(chunks, rs) * WG_ROWS;
   *n_rs = (int)ceil_div(n_out, *rows_per_rs);
@@ -244,7 +210,7 @@ int osb_conv_wgrad_tc(const void *x_split, int32_t cin, int64_t n_in, const int3
   k_conv_wgrad_tc<<<(unsigned)units, WG_THREADS, smem_bytes, stream>>>(tmG, p);
   OSB_LAUNCH_CHECK();
   const int64_t total = (int64_t)K * cin * cout;
-  k_conv_wgrad_reduce<<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 148 * 8), 256, 0, stream>>>(p.partial, K, cin, cout, p.n_mt, p.n_nt,
+  k_conv_wgrad_reduce<<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 132 * 8), 256, 0, stream>>>(p.partial, K, cin, cout, p.n_mt, p.n_nt,
                                                                                                      p.n_rs, gw);
   OSB_LAUNCH_CHECK();
   return 0;

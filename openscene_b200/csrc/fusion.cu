@@ -176,7 +176,7 @@ int osb_fusion_accumulate(const void *points, int32_t points_is_f64, int64_t n, 
   OSB_LAUNCH_CHECK();
   if (sum != nullptr) {     // mapping-only calls pass sum == nullptr
     OSB_CHECK(counter != nullptr, "osb_fusion_accumulate: counter is null");
-    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(n, 8), 148 * 16);
+    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(n, 8), 132 * 16);
     k_fusion_gather<<<blocks, 256, 0, stream>>>(pix, n, n_frames, (const __half *)feat, (int64_t)H * W * C, C, sum, counter);
     OSB_LAUNCH_CHECK();
   }
@@ -187,7 +187,7 @@ int osb_fusion_finalize(const float *sum, const float *counter, int64_t n, int32
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(C > 0 && C % 4 == 0, "osb_fusion_finalize: feature width %d must be a multiple of 4", C);
   if (n == 0) return 0;
-  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(n * (C / 4), 256), 148 * 16);
+  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(n * (C / 4), 256), 132 * 16);
   k_fusion_finalize<<<blocks, 256, 0, stream>>>(sum, counter, n, C, feat_bank);
   OSB_LAUNCH_CHECK();
   return 0;

@@ -142,7 +142,7 @@ static bool use_simt() {   // OSB_MATCH_SIMT=1 selects the CUDA-core kernels bel
 }
 
 static unsigned match_grid(int64_t n_pts) {
-  return (unsigned)std::min<int64_t>(ceil_div(n_pts, 8), 148 * 8);
+  return (unsigned)std::min<int64_t>(ceil_div(n_pts, 8), 132 * 8);
 }
 
 }  // namespace osb
@@ -248,7 +248,7 @@ extern "C" int osb_folded_head_finish(const float *z, int64_t n, int32_t ld, int
                                       int64_t *label, float *smax, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(n > 0 && c_norm > 0 && k_text > 0 && ld >= c_norm + k_text, "osb_folded_head_finish: bad shape");
-  const unsigned grid = (unsigned)std::min<int64_t>(osb::ceil_div(n, 8), 148 * 8);
+  const unsigned grid = (unsigned)std::min<int64_t>(osb::ceil_div(n, 8), 132 * 8);
   osb::k_folded_head_finish<<<grid, 256, 0, stream>>>(z, n, ld, c_norm, k_text, (__half *)scores_f16, label, smax);
   OSB_LAUNCH_CHECK();
   return 0;

@@ -1,4 +1,4 @@
-// Open-vocabulary matching on 5th-gen tensor cores (run/evaluate.py:288-323).
+// Open-vocabulary matching on tensor cores (wgmma) (run/evaluate.py:288-323).
 //
 //   scores[p, k] = fp16( sum_c a[p, c] * text[k, c] ),  a[p,:] = fp16( prep(feat[v(p), :]) ),  fp32 accumulation
 //
@@ -10,9 +10,9 @@
 // One CTA = 128 points.  Warps 0-15 build the A operand: one warp per row at a time, the row lives in registers
 // (coalesced 256-byte loads), is reduced for the norm, rounded to fp16 and written into the K-major 128B-swizzled
 // shared-memory tile of all C/64 depth chunks (192 KB for C = 768).  Warp 16 streams the text matrix chunk by chunk with
-// TMA (rows >= K_text are out of bounds -> zero fill), warp 17 issues `tcgen05.mma kind::f16` (M=128, N<=96 per pass,
-// K=16), warps 0-3 read the accumulators from TMEM, round to fp16, take the first-maximum argmax and write
-// scores / labels / row maxima.  HBM-bound: 4*C (or 2*C) bytes per point against 2*C*K flops.
+// TMA (rows >= K_text are out of bounds -> zero fill).  Warps 0-7 (two warpgroups, 64 points each) then run `wgmma` f16
+// (M=64, N=96 per pass, K=16) into register accumulators, round to fp16, keep the first-maximum argmax over the passes and
+// write scores / labels / row maxima.  HBM-bound: 4*C (or 2*C) bytes per point against 2*C*K flops.
 #include "tc_ptx.cuh"
 #include <algorithm>
 
@@ -21,7 +21,7 @@ namespace osb {
 constexpr int MT_M = 128;
 constexpr int MT_NW = 96;            // text rows per MMA pass (N of the instruction)
 constexpr int MT_PW = 16;             // A-producer warps (8 rows each)
-constexpr int MT_THREADS = (MT_PW + 2) * 32;   // + TMA warp + MMA warp
+constexpr int MT_THREADS = (MT_PW + 1) * 32;   // + TMA warp
 constexpr int MT_BSTAGES = 2;
 
 struct MatchTcParams {
@@ -30,17 +30,13 @@ struct MatchTcParams {
   const float *sel_a, *sel_b;        // ensemble: use feat2 where sel_a[p] < sel_b[p]
   const int64_t *inds_reverse;       // [n_pts] or NULL
   int64_t n_pts;
-  int C, k_text, n_pass, tmem_cols;
+  int C, k_text, n_pass;
   int feat_is_f16, normalize;
   __half *scores;                    // [n_pts, k_text] or NULL
   int64_t *label;                    // [n_pts] or NULL
   float *smax;                       // [n_pts] or NULL
   __half *feat_out;                  // [n_pts, C] or NULL: the fp16 operand actually multiplied (ensemble feature)
 };
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t acc) {
-  umma_bf16(tmem_d, desc_a, desc_b, idesc, acc);      // same instruction; operand format comes from the descriptor
-}
 
 template <int NP>   // half2 pairs per lane: C = 64 * NP
 __global__ void __launch_bounds__(MT_THREADS, 1)
@@ -51,28 +47,20 @@ k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
   constexpr int A_BYTES = NP * MT_M * 128;                      // NP chunks of [128 rows x 128 B]
   constexpr int B_BYTES = MT_NW * 128;
   uint8_t *sA = smem, *sB = smem + A_BYTES;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(sB + MT_BSTAGES * B_BYTES);   // b_full[2], b_empty[2], a_full, accum
-  uint32_t *s_misc = reinterpret_cast<uint32_t *>(bars + 8);
+  uint64_t *bars = reinterpret_cast<uint64_t *>(sB + MT_BSTAGES * B_BYTES);   // b_full[2], b_empty[2], a_full
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int64_t row0 = (int64_t)blockIdx.x * MT_M;
-  const uint32_t b_full = smem_u32(bars), b_empty = smem_u32(bars + 2), a_full = smem_u32(bars + 4), accum = smem_u32(bars + 5);
+  const uint32_t b_full = smem_u32(bars), b_empty = smem_u32(bars + 2), a_full = smem_u32(bars + 4);
 
   if (tid == 0) {
-    for (int s = 0; s < MT_BSTAGES; ++s) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, 1); }
+    // b_empty: one arrival per consumer warpgroup
+    for (int s = 0; s < MT_BSTAGES; ++s) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, 2); }
     mbar_init(a_full, MT_PW * 32);
-    mbar_init(accum, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MT_PW + 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_misc[0])), "r"((uint32_t)p.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == MT_PW * 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmT) : "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = s_misc[0];
   const int n_stage = p.n_pass * NP;
 
   if (warp < MT_PW) {
@@ -151,7 +139,7 @@ k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
         }
       }
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic-proxy writes -> UMMA reads
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic-proxy writes -> wgmma reads
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a_full) : "memory");
   } else if (warp == MT_PW) {
     // ============================ TMA producer: text chunks ==================================
@@ -166,62 +154,69 @@ k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
       __syncwarp();
       if (++s == MT_BSTAGES) { s = 0; phase ^= 1; }
     }
-  } else {
-    // ============================ MMA issuer ==================================================
-    // instruction descriptor: D=f32, A=B=f16 (format 0), K-major both, N = 96, M = 128
-    const uint32_t idesc = (1u << 4) | ((uint32_t)(MT_NW >> 3) << 17) | ((uint32_t)(MT_M >> 4) << 24);
-    mbar_wait(a_full, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    int s = 0; uint32_t phase = 0;
-    for (int t = 0; t < n_stage; ++t) {
-      const int pass = t / NP, c = t % NP;
-      mbar_wait(b_full + 8 * s, phase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint64_t da = umma_desc(smem_u32(sA + c * (MT_M * 128))), db = umma_desc(smem_u32(sB + s * B_BYTES));
-#pragma unroll
-        for (int h = 0; h < 4; ++h)      // 64 fp16 per chunk = 4 K-steps of 16 (32 bytes each)
-          umma_f16(tmem_base + pass * MT_NW, da + 2 * h, db + 2 * h, idesc, (c > 0 || h > 0) ? 1u : 0u);
-        umma_commit(b_empty + 8 * s);
-      }
-      __syncwarp();
-      if (++s == MT_BSTAGES) { s = 0; phase ^= 1; }
-    }
-    if (elect_one()) umma_commit(accum);
-    __syncwarp();
   }
 
-  if (warp < 4) {
-    // ============================ epilogue: fp16 rounding, argmax =============================
-    mbar_wait(accum, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int64_t pt = row0 + warp * 32 + lane;
-    float best = -INFINITY;
-    int best_k = 0;
-    for (int col = 0; col < p.n_pass * MT_NW; col += 16) {
-      if (col >= p.k_text) break;                                   // warp-uniform
-      uint32_t a[16];
-      tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + col, a);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  if (warp < 8) {
+    // ============ wgmma: warpgroup g multiplies points [64g, 64g + 64), pass by pass; fp16 rounding, argmax ============
+    const int g = warp >> 2;
+    const int r_lo = 64 * g + 16 * (warp & 3) + (lane >> 2);      // this thread's rows: r_lo and r_lo + 8
+    const int cq = 2 * (lane & 3);
+    float best[2] = {-INFINITY, -INFINITY};
+    int best_k[2] = {0, 0};
+    mbar_wait(a_full, 0);
+    int s = 0; uint32_t phase = 0;
+    for (int pass = 0; pass < p.n_pass; ++pass) {
+      float acc[MT_NW / 2];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int k = col + j;
-        if (k < p.k_text) {
-          const __half h = __float2half_rn(__uint_as_float(a[j]));
-          const float sc = __half2float(h);
-          if (p.scores != nullptr && pt < p.n_pts) p.scores[pt * p.k_text + k] = h;
-          if (sc > best) { best = sc; best_k = k; }
+      for (int i = 0; i < MT_NW / 2; ++i) acc[i] = 0.f;
+      for (int c = 0; c < NP; ++c) {
+        mbar_wait(b_full + 8 * s, phase);
+        const uint64_t da = gmma_desc(smem_u32(sA + c * (MT_M * 128) + g * 64 * 128)), db = gmma_desc(smem_u32(sB + s * B_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {    // 64 fp16 per chunk = 4 K-steps of 16 (32 bytes each)
+          wgmma_n64_f16<0, 0>(acc, da + 2 * h, db + 2 * h, 1u);
+          wgmma_n32_f16<0, 0>(acc + 32, da + 2 * h, db + 2 * h + 512, 1u);
         }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_hold(acc);
+        if ((tid & 127) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(b_empty + 8 * s) : "memory");
+        if (++s == MT_BSTAGES) { s = 0; phase ^= 1; }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t pt = row0 + r_lo + 8 * h;
+#pragma unroll
+        for (int i = 0; i < MT_NW / 8; ++i)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int k = pass * MT_NW + 8 * i + cq + e;       // ascending per thread: the first maximum is kept
+            if (k < p.k_text) {
+              const __half hv = __float2half_rn(acc[4 * i + 2 * h + e]);
+              const float sc = __half2float(hv);
+              if (p.scores != nullptr && pt < p.n_pts) p.scores[pt * p.k_text + k] = hv;
+              if (sc > best[h]) { best[h] = sc; best_k[h] = k; }
+            }
+          }
       }
     }
-    if (pt < p.n_pts) {
-      if (p.label) p.label[pt] = best_k;
-      if (p.smax) p.smax[pt] = best;
+    // the four lanes of a row hold interleaved column pairs: the maximum with the smallest column wins
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int o = 1; o < 4; o <<= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best[h], o);
+        const int ok = __shfl_xor_sync(0xffffffffu, best_k[h], o);
+        if (ob > best[h] || (ob == best[h] && ok < best_k[h])) { best[h] = ob; best_k[h] = ok; }
+      }
+      const int64_t pt = row0 + r_lo + 8 * h;
+      if ((lane & 3) == 0 && pt < p.n_pts) {
+        if (p.label) p.label[pt] = best_k[h];
+        if (p.smax) p.smax[pt] = best[h];
+      }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == MT_PW + 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols));
 }
 
 static int launch_match_tc(const MatchTcParams &p, const void *text_f16, cudaStream_t stream) {
@@ -248,9 +243,7 @@ int match_tc_run(const void *feat, int feat_is_f16, const void *feat2_f16, const
   p.feat = feat; p.feat2 = (const __half *)feat2_f16; p.sel_a = sel_a; p.sel_b = sel_b;
   p.inds_reverse = inds_reverse; p.n_pts = n_pts; p.C = c; p.k_text = k_text;
   p.n_pass = (k_text + MT_NW - 1) / MT_NW;
-  OSB_CHECK(p.n_pass * MT_NW <= 512, "match: K_text=%d too large for one TMEM allocation", k_text);
-  p.tmem_cols = 32;
-  while (p.tmem_cols < p.n_pass * MT_NW) p.tmem_cols <<= 1;
+  OSB_CHECK(p.n_pass * MT_NW <= 512, "match: K_text=%d too large (at most 512 text rows)", k_text);
   p.feat_is_f16 = feat_is_f16; p.normalize = normalize;
   p.scores = (__half *)scores_f16; p.label = label; p.smax = smax; p.feat_out = (__half *)feat_out_f16;
   return launch_match_tc(p, text_f16, stream);

@@ -82,7 +82,7 @@ int osb_confusion_accumulate(const void *pred, const void *gt, int32_t labels_ar
   const size_t smem = (size_t)(num_classes + 1) * (num_classes + 1) * sizeof(uint32_t);
   const int use_smem = smem <= kMetricSmemMax;
   // a block's uint32 bins must not overflow: every block sees at most ceil(n / grid) * ... < 2^32 items for n < 2^40
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, 256 * 8), 148 * 4);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, 256 * 8), 132 * 4);
   auto *conf = reinterpret_cast<unsigned long long *>(confusion);
   if (labels_are_i64) {
     if (use_smem) OSB_CUDA(cudaFuncSetAttribute(k_confusion<int64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMetricSmemMax));
@@ -105,7 +105,7 @@ int osb_intersection_union(const void *output, const void *target, int32_t label
   if (n == 0) return 0;
   const size_t smem = (size_t)3 * K * sizeof(uint32_t);
   const int use_smem = smem <= 48 * 1024;
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, 256 * 8), 148 * 4);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, 256 * 8), 132 * 4);
   auto *a = reinterpret_cast<unsigned long long *>(areas);
   if (labels_are_i64)
     k_inter_union<int64_t><<<grid, 256, use_smem ? smem : 0, stream>>>((const int64_t *)output, (const int64_t *)target, n, K, ignore_id, a, use_smem);

@@ -96,7 +96,7 @@ int osb_feature_remap(const uint8_t *mask_full, int64_t n_pts, const int64_t *vo
   OSB_CUDA(cudaStreamSynchronize(stream));
   OSB_CHECK(h[2] == 0, "osb_feature_remap: %d voxel indices outside 0..n_pts-1", h[2]);
   OSB_CHECK((int64_t)h[0] == m_rows, "osb_feature_remap: feat has %lld rows but mask_full has %d True entries", (long long)m_rows, h[0]);
-  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(n_vox, 8), 148 * 16);
+  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(n_vox, 8), 132 * 16);
   k_remap_rows<<<blocks, 256, 0, stream>>>(vox_ind, n_vox, mask_vox, rank1, pos1, (const uint8_t *)feat, row_bytes, keep_all, (uint8_t *)feat_out);
   OSB_LAUNCH_CHECK();
   *n_out_host = keep_all ? n_vox : (int64_t)h[1];

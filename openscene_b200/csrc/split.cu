@@ -1,4 +1,4 @@
-// fp32 <-> split-bf16 rows (the activation layout of the tcgen05 path, see include/osb200.h).
+// fp32 <-> split-bf16 rows (the activation layout of the tensor-core path, see include/osb200.h).
 #include "common.cuh"
 #include <algorithm>
 
@@ -49,7 +49,7 @@ int osb_f32_to_split(const float *in, int64_t n, int32_t c, void *out_split, voi
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(c > 0 && c % 32 == 0, "osb_f32_to_split: channels (%d) must be a multiple of 32", c);
   if (n == 0) return 0;
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n * (c / 8), 256), 148 * 16);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n * (c / 8), 256), 132 * 16);
   k_f32_to_split<<<grid, 256, 0, stream>>>(in, n, c, (uint8_t *)out_split);
   OSB_LAUNCH_CHECK();
   return 0;
@@ -59,7 +59,7 @@ int osb_split_to_f32(const void *in_split, int64_t n, int32_t c, float *out, voi
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(c > 0 && c % 32 == 0, "osb_split_to_f32: channels (%d) must be a multiple of 32", c);
   if (n == 0) return 0;
-  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n * (c / 8), 256), 148 * 16);
+  const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n * (c / 8), 256), 132 * 16);
   k_split_to_f32<<<grid, 256, 0, stream>>>((const uint8_t *)in_split, n, c, out);
   OSB_LAUNCH_CHECK();
   return 0;

@@ -55,7 +55,7 @@ class _Conv:
         self.wpack_a = self.wpack.data_ptr() if self.wpack is not None else 0
         self.wtiles = tc.pack_weight_tiles(w3) if self.wpack is not None else None        # persistent-kernel packing
         self.wtiles_a = self.wtiles.data_ptr() if self.wtiles is not None else 0
-        self.n_ntiles = max(1, -(-self.cout // 256))
+        self.n_ntiles = max(1, -(-self.cout // 128))
         self.scale_a = self.scale.data_ptr() if self.scale is not None else 0
         self.shift_a = self.shift.data_ptr() if self.shift is not None else 0
 
@@ -122,7 +122,7 @@ class FusedMinkUNet:
                     up.wpack_a = up.wpack.data_ptr()
                     up.wtiles = tc.pack_weight_tiles(wide)
                     up.wtiles_a = up.wtiles.data_ptr()
-                    up.n_ntiles = max(1, -(-(up.K * up.cout) // 256))
+                    up.n_ntiles = max(1, -(-(up.K * up.cout) // 128))
                 self.dec.append((up, self._blocks(getattr(net, f'block{j + 1}'))))
             self.final = _Conv(net.final, None, keep_f32=True)
         self._sig = self._signature()
@@ -164,7 +164,7 @@ class FusedMinkUNet:
         ch = self._chain
         if self.layer_log is not None:
             self.layer_log.append((n_rows, K, c0 + c1, cout, 'dense-up' if cmap_a else ('res' if res_a else '')))
-        tiles = -(-n_rows // 128) * max(1, -(-cout // 256))
+        tiles = -(-n_rows // 128) * max(1, -(-cout // 128))
         small = tiles <= self._chain_small
         if not (small and self._chain_prev_small):
             ch.cut()
@@ -342,7 +342,7 @@ class FusedMinkUNet:
         cv.wtiles = tc.pack_weight_tiles(w)
         cv.scale = cv.shift = None
         cv.wpack_a, cv.wtiles_a, cv.scale_a, cv.shift_a = cv.wpack.data_ptr(), cv.wtiles.data_ptr(), 0, 0
-        cv.n_ntiles = max(1, -(-cout // 256))
+        cv.n_ntiles = max(1, -(-cout // 128))
         return (cv, cin, k, self._signature())               # the signature lets forward_scores refuse a head folded from older weights
 
     @torch.no_grad()

@@ -1,4 +1,4 @@
-"""The ``MinkowskiEngine`` surface OpenScene uses, re-implemented over ``libosb200`` (sm_100a).
+"""The ``MinkowskiEngine`` surface OpenScene uses, re-implemented over ``libosb200`` (sm_90a).
 
 Importable as ``MinkowskiEngine`` (the top-level ``MinkowskiEngine/`` package re-exports this
 module) so that the reference's ``models/mink_unet.py``, ``models/resnet_base.py``,
@@ -258,7 +258,7 @@ def _tc_ok(cin, cout, K):
 
 
 def _conv_tc_split(xs, kmap, wpack, cin, cout, K, n_out):
-    """split rows in, fp32 rows out through the tcgen05 kernel (bf16x3 split operands)."""
+    """split rows in, fp32 rows out through the tensor-core kernel (bf16x3 split operands)."""
     from . import tc
     nbr = kmap.nbr if kmap is not None else None
     return tc.conv_tc(xs, cin, None, 0, nbr, n_out, K, wpack, cout, out_split=False, out_f32=True)[1]
@@ -267,7 +267,7 @@ def _conv_tc_split(xs, kmap, wpack, cin, cout, K, n_out):
 class SparseConvFunction(torch.autograd.Function):
     """Forward / dgrad / wgrad of the generalised sparse convolution on libosb200 kernels
     (replaces MinkowskiConvolutionFunction / ...TransposeFunction inside MinkowskiEngine; run/distill.py:321,333).
-    With channel counts that are multiples of 32 all three run on tensor cores: forward and dgrad on the tcgen05
+    With channel counts that are multiples of 32 all three run on tensor cores: forward and dgrad on the tensor-core
     convolution kernel (dgrad = the same kernel on the transposed map with W^T packed), wgrad on csrc/conv_wgrad_tc.cu.
     The input is saved in the split-bf16 layout the kernels read (the conversion is paid once, in forward); packed weights
     are memoised on the parameter's version counter.  Odd shapes use the exact-fp32 CUDA-core kernels."""
@@ -363,7 +363,7 @@ class _ConvBase(nn.Module):
         return self.kernel.unsqueeze(0) if self.kernel.dim() == 2 else self.kernel
 
     def _run_conv(self, input, kmap, n_out):
-        """Inference (grad disabled) with channel counts that are multiples of 32 runs on the tcgen05 kernel
+        """Inference (grad disabled) with channel counts that are multiples of 32 runs on the tensor-core kernel
         (bf16x3 split operands, ~1e-5 relative); everything else on the exact-fp32 kernels with autograd."""
         x = input._F
         K = self.kernel_volume if not self.use_mm else 1

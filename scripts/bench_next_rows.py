@@ -21,7 +21,7 @@ def peak_gbs():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'data sheet (H100 SXM HBM3, 700 W card), not measured'
 
 
 def timed(fn, reps=10, warm=3):

@@ -1,4 +1,4 @@
-"""GPU micro-benchmark of the tcgen05 sparse-conv kernel on the config-2 scene (tuning aid, not a bench line).
+"""GPU micro-benchmark of the tensor-core sparse-conv kernel on the config-2 scene (tuning aid, not a bench line).
 Prints microseconds per launch for a few shapes under different pipeline settings."""
 import os
 import sys
@@ -46,7 +46,7 @@ def case(level, cin, cout, ks, label, **dbg):
     tc.debug_set_tc(**dbg)
     f32 = cout > 256
     us = timeit(lambda: tc.conv_tc(x, cin, None, 0, nbr, n, K, w, cout, None, None, None, True, not f32, f32, None))
-    tc.debug_set_tc(use_gather4=2, smem_budget=112 * 1024, dbg_skip=0, force_split=0, target_ctas=148, pf_dist=0, small_nt=0, min_stages=3, lazy=1)
+    tc.debug_set_tc(use_gather4=2, smem_budget=227 * 1024, dbg_skip=0, force_split=0, target_ctas=132, pf_dist=0, small_nt=0, min_stages=3, lazy=1)
     print(f'{label:46s} L{level} n={n:7d} {cin:3d}->{cout:3d} k{ks}  {us:9.1f} us', flush=True)
 
 
@@ -59,15 +59,15 @@ if len(sys.argv) > 2 and sys.argv[2] == 'lazy':
 if len(sys.argv) > 2 and sys.argv[2] == 'occ':
     B3, B4 = 75 * 1024, 56 * 1024
     for (lvl, cin, cout, ks) in ((1, 64, 64, 3), (1, 192, 96, 3), (1, 96, 96, 3), (0, 96, 96, 3), (0, 128, 96, 3), (0, 96, 96, 1), (2, 128, 128, 3), (0, 32, 32, 2)):
-        case(lvl, cin, cout, ks, '2 CTA/SM x 3 stages')
-        case(lvl, cin, cout, ks, '3 CTA/SM x 2 stages', smem_budget=B3, min_stages=2)
-        case(lvl, cin, cout, ks, '4 CTA/SM x 2 stages (if fits)', smem_budget=B4, min_stages=2)
+        case(lvl, cin, cout, ks, 'default smem budget')
+        case(lvl, cin, cout, ks, '75 KB smem budget, 2 stages', smem_budget=B3, min_stages=2)
+        case(lvl, cin, cout, ks, '56 KB smem budget, 2 stages', smem_budget=B4, min_stages=2)
     sys.exit(0)
 if len(sys.argv) > 2 and sys.argv[2] == 'small':
     for lvl in (2, 3, 4):
         c = {2: 128, 3: 256, 4: 256}[lvl]
         for snt in (0, 128, 64):
-            for tgt in (148, 296):
+            for tgt in (132, 264):
                 case(lvl, c, c, 3, f'L{lvl} small_nt={snt} target={tgt}', small_nt=snt, target_ctas=tgt)
         case(lvl, c, c, 1, f'L{lvl} 1x1 small_nt=0', small_nt=0)
         case(lvl, c, c, 1, f'L{lvl} 1x1 small_nt=64', small_nt=64)
@@ -75,17 +75,16 @@ if len(sys.argv) > 2 and sys.argv[2] == 'small':
 if len(sys.argv) > 2 and sys.argv[2] == 'pf':
     for hot in (False, True):
         HOT = hot
-        for pf in (0, 148, 296, 444, 592):
+        for pf in (0, 132, 264, 396, 528):
             case(0, 96, 96, 3, f'hot={hot} pf_dist={pf}', pf_dist=pf)
-        case(0, 96, 96, 3, f'hot={hot} pf 296, 1 CTA/SM', pf_dist=148, smem_budget=B1)
+        case(0, 96, 96, 3, f'hot={hot} pf 132, budget B1', pf_dist=132, smem_budget=B1)
         case(0, 128, 96, 3, f'hot={hot} 128->96 pf 296', pf_dist=296)
         case(0, 96, 96, 1, f'hot={hot} 1x1 pf 0', pf_dist=0)
         case(0, 96, 96, 1, f'hot={hot} 1x1 pf 296', pf_dist=296)
         case(0, 96, 768, 1, f'hot={hot} final pf 0', pf_dist=0)
         case(0, 96, 768, 1, f'hot={hot} final pf 296', pf_dist=296)
     sys.exit(0)
-case(0, 96, 96, 3, 'base (2 CTA/SM, cp.async)')
-case(0, 96, 96, 3, 'TMA gather4', use_gather4=1)
+case(0, 96, 96, 3, 'base (default smem budget, cp.async)')
 case(0, 96, 96, 3, '1 CTA/SM deep pipeline', smem_budget=B1)
 case(0, 96, 96, 3, 'no A gathers (timing only)', dbg_skip=1)
 case(0, 96, 96, 3, 'no B loads (timing only)', dbg_skip=2)
@@ -100,4 +99,4 @@ for lvl, tag in ((1, 'L1 64->64'), (2, 'L2'), (3, 'L3'), (4, 'L4')):
     case(lvl, c, c, 3, f'{tag} heuristic split')
     case(lvl, c, c, 3, f'{tag} no split', force_split=1)
     case(lvl, c, c, 3, f'{tag} target 592 CTAs', target_ctas=592)
-    case(lvl, c, c, 3, f'{tag} target 148 CTAs', target_ctas=148)
+    case(lvl, c, c, 3, f'{tag} target 132 CTAs', target_ctas=132)

@@ -43,7 +43,7 @@ def run(cin, cout, ks, label, clock=False, **dbg):
             *np.median(d, axis=0), np.median(c[:, 5] - c[:, 0]))
         # concurrency: CTAs alive per SM over time is not observable here; report span of the whole grid instead
         msg += '  grid-span %.0f cycles' % (c[:, 5].max() - c[:, 0].min())
-    tc.debug_set_tc(use_gather4=2, smem_budget=112 * 1024, dbg_skip=0, force_split=0, target_ctas=296, pf_dist=0)
+    tc.debug_set_tc(use_gather4=2, smem_budget=227 * 1024, dbg_skip=0, force_split=0, target_ctas=264, pf_dist=0)
     print(msg, flush=True)
 
 

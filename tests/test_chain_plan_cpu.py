@@ -2,8 +2,8 @@
 
 ``osb_conv_desc_fill`` / ``osb_conv_chain_workspace_bytes`` are pure host functions: they choose the tile shape, the
 split factor and the stage partition of a layer and validate the arguments.  The kernel then derives every role's loop
-from those few integers, so the invariants below are what keeps the roles (weight producer, two MMA issuers, gather warps,
-epilogue) walking the same sequence of items: a violation would be a hang or a silently skipped unit on the device.
+from those few integers, so the invariants below are what keeps the roles (weight producer, gather warps, two consumer
+warpgroups) walking the same sequence of items: a violation would be a hang or a silently skipped unit on the device.
 The walk itself (``_items``) restates the kernel's ``CH_FOR_ITEMS`` macro; the descriptor numbers come from the library."""
 import ctypes
 import struct
@@ -72,10 +72,10 @@ def test_descriptor_invariants(n_out, K, c0, c1, cout):
     assert d is not None, err
     T = K * (c0 + c1) // 32
     assert (d['K'], d['nb0'], d['nb1'], d['cout'], d['n_out']) == (K, c0 // 32, c1 // 32, cout, n_out)
-    # tile shape: the padded width is whole N tiles of at most 256 columns (TMEM: 2 buffers x 256 columns); two row tiles
-    # share a weight tile only when both accumulators fit one buffer
-    assert d['cout_pad'] >= cout and d['cout_pad'] == d['nt'] * d['n_ntiles'] and d['nt'] <= 256 and d['nt'] % 16 == 0
-    assert d['nsub_max'] == (2 if d['nt'] <= 128 else 1)
+    # tile shape: the padded width is whole N tiles of at most 128 columns; two row tiles share a weight tile only when the
+    # N tile is at most 64 wide (a consumer thread then holds at most 64 fp32 accumulators)
+    assert d['cout_pad'] >= cout and d['cout_pad'] == d['nt'] * d['n_ntiles'] and d['nt'] <= 128 and d['nt'] % 16 == 0
+    assert d['nsub_max'] == (2 if d['nt'] <= 64 else 1)
     assert d['m_tiles'] == -(-n_out // 128)
     # stage partition: splits tile [0, T) without an empty one
     ns, sps = d['nsplit'], d['stages_per_split']
@@ -119,7 +119,7 @@ def test_split_factor_rules():
             assert d['nsplit'] == 1, (n_out, K, c0, c1, cout)
         if K * (c0 + c1) // 32 == 1:
             assert d['nsplit'] == 1
-    d, _ = _fill(473, 27, 256, 0, 256)            # 4 tiles x 216 stages: split as far as the cap allows
+    d, _ = _fill(473, 27, 256, 0, 256)            # 8 tiles x 216 stages: split as far as the cap allows
     assert d['nsplit'] >= 16
     L = C.lib()
     assert L.osb_tuning_set(b'chain_force_split', 1) == 0
@@ -134,7 +134,7 @@ def test_split_factor_rules():
 def test_dense_transposed_form():
     d, err = _fill(40640, 1, 128, 0, 8 * 96, cmap=FAKE, cmap_cout=96, nbr=0)
     assert d is not None, err
-    assert d['nsplit'] == 1 and d['cmap_cout'] == 96 and d['cout_pad'] == 768 and d['nt'] == 256 and d['n_ntiles'] == 3
+    assert d['nsplit'] == 1 and d['cmap_cout'] == 96 and d['cout_pad'] == 768 and d['nt'] == 128 and d['n_ntiles'] == 6
 
 
 @pytest.mark.parametrize('kw,msg', [

@@ -1,19 +1,19 @@
 """Randomised model of the synchronisation protocol of the persistent convolution kernel (csrc/conv_chain.cu), no GPU.
 
 The kernel's twelve warps talk through mbarriers whose waiters see only a phase PARITY, with three asynchronous agents in
-between (cp.async row copies, bulk weight copies, the tensor pipe with tcgen05.commit).  What can go wrong is ordering, not
+between (cp.async row copies, bulk weight copies, each consumer warpgroup's wgmma groups).  What can go wrong is ordering, not
 arithmetic: a producer that passes a parity test one lap early overwrites rows that have not been multiplied, a consumer
 that mistakes "lap L-2 filled" for "lap L filled" multiplies stale rows, a role that skips an arrival hangs the CTA.  This
-file restates the protocol -- every wait, arrival and slot / phase update of the five roles, in the order the kernel performs
+file restates the protocol -- every wait, arrival and slot / phase update of the three roles, in the order the kernel performs
 them -- as coroutines over modelled mbarriers, runs it under random schedules (including arbitrarily late completion of
 copies and MMAs) and checks that
 
-  * every schedule terminates (no deadlock),
+  * every schedule terminates (no deadlock; a consumer holds the slots of two stages: it frees a stage after wgmma_wait<1>),
   * every MMA reads exactly the row slot and weight slot contents meant for it (stage, sub-tile, item),
   * no row / weight slot is overwritten while an issued MMA still has to read it,
-  * an accumulator buffer is drained only after all MMAs of its item, and reused only after all four epilogue warps left it.
+  * a consumer warpgroup's epilogue runs only after all MMAs of its item retired.
 
-The two rules DESIGN.md §4 calls "learnt the hard way" are visible here: with ring slots dealt round-robin over the gather
+The reason every ring slot has a fixed owner is visible here: with ring slots dealt round-robin over the gather
 warps (the first version) the same model finds overwritten rows within a few schedules -- the negative control below.
 It is a model of the PROTOCOL: what the hardware does inside one instruction (the proxy fences, the swizzle, the descriptors)
 is covered by the GPU tests (tests/test_gpu_conv_chain.py: bit-identical repeated launches against the fp64 oracle)."""
@@ -21,7 +21,7 @@ import random
 
 import pytest
 
-A_WARPS = 5                     # CH_A_WARPS
+A_WARPS = 3                     # CH_A_WARPS
 
 
 class Bar:
@@ -57,23 +57,20 @@ class Violation(AssertionError):
 
 
 class Cta:
-    def __init__(self, items, sa, sb, rng, fixed_owners=True, layer_ends=()):
-        self.items, self.sa, self.sb, self.rng = items, sa, sb, rng
+    def __init__(self, items, sa, sb, rng, fixed_owners=True, layer_ends=(), a_warps=A_WARPS):
+        self.items, self.sa, self.sb, self.rng, self.a_warps = items, sa, sb, rng, a_warps
         self.fixed_owners, self.layer_ends = fixed_owners, set(layer_ends)
         self.fullA = [Bar(1) for _ in range(sa)]            # (32 lane arrivals in the kernel: one modelled completion)
-        self.emptyA = [Bar(1) for _ in range(sa)]
+        self.emptyA = [Bar(2) for _ in range(sa)]           # one arrival per consumer warpgroup
         self.fullB = [Bar(1) for _ in range(sb)]
-        self.emptyB = [Bar(2) for _ in range(sb)]           # one arrival per issuer
-        self.accFull = [Bar(2) for _ in range(2)]
-        self.accEmpty = [Bar(4) for _ in range(2)]
+        self.emptyB = [Bar(2) for _ in range(sb)]           # one arrival per consumer warpgroup
         self.slotA = [None] * sa                            # content tags
         self.slotB = [None] * sb
-        self.readsA = [0] * sa                              # issued MMAs that still have to read the slot
+        self.readsA = [0] * sa                              # issued wgmmas (either warpgroup) that still have to read the slot
         self.readsB = [0] * sb
-        self.acc = [dict(item=None, done=0, readers=0) for _ in range(2)]
         self.fifo = {}                                      # async agents: name -> list of pending operations (in order)
         self.sync_wait = {}                                 # layer boundary (__syncthreads): role -> layer index reached
-        self.n_roles = 1 + 2 + A_WARPS + 4
+        self.n_roles = 1 + a_warps + 2
 
     # ---- asynchronous agents -------------------------------------------------------------------
     def push(self, agent, op):
@@ -104,74 +101,65 @@ class Cta:
                 yield None
             yield from self.layer_sync('weights', it)
 
-    def issuer(self, mi):
-        a_slot = a_phase = b_slot = b_phase = n_item = 0
+    def consumer(self, g):
+        """chain_item: per stage wait for its slots, issue one wgmma group, wgmma_wait<1>, free the PREVIOUS stage's slots;
+        after the item wgmma_wait<0>, free the last stage's slots, epilogue."""
+        a_slot = a_phase = b_slot = b_phase = 0
         sa, sb = self.sa, self.sb
-        pipe = f'tensor{mi}'
+        pipe = f'tensor{g}'
         for it, (nsub, stages) in enumerate(self.items):
-            buf = n_item & 1
-            mine = mi < nsub
-            yield (self.accEmpty[buf], ((n_item >> 1) & 1) ^ 1)
-            t = 0
-            while t < stages:
-                nst = min(2, stages - t)
-                sl, sph, bs, bph = [], [], [], []
-                as_, ap_, bs_, bp_ = a_slot + mi, a_phase, b_slot, b_phase
-                if as_ >= sa:
-                    as_, ap_ = as_ - sa, ap_ ^ 1
-                for _ in range(2):
-                    sl.append(as_); sph.append(ap_); bs.append(bs_); bph.append(bp_)
-                    as_ += nsub
-                    if as_ >= sa:
-                        as_, ap_ = as_ - sa, ap_ ^ 1
-                    bs_ += 1
-                    if bs_ == sb:
-                        bs_, bp_ = 0, bp_ ^ 1
-                if mine:
-                    for jx in range(nst):                   # all barriers of the batch (the kernel probes them together)
-                        yield (self.fullB[bs[jx]], bph[jx])
-                        yield (self.fullA[sl[jx]], sph[jx])
-                    for jx in range(nst):
-                        a, b, want_a, want_b = sl[jx], bs[jx], (it, t + jx, mi), (it, t + jx)
-                        self.readsA[a] += 1
-                        self.readsB[b] += 1
-                        first = (jx == 0 and t == 0)
+            acc = dict(done=0)
+            prev = None                                        # (row slots, weight slot, group-retired marker) of the last stage
+            for t in range(stages):
+                rows, phases = [a_slot], [a_phase]
+                if nsub == 2:
+                    a1, p1 = a_slot + 1, a_phase
+                    if a1 >= sa:
+                        a1, p1 = a1 - sa, p1 ^ 1
+                    rows.append(a1); phases.append(p1)
+                yield (self.fullB[b_slot], b_phase)            # (the kernel probes all of them together)
+                for a, p in zip(rows, phases):
+                    yield (self.fullA[a], p)
+                b = b_slot
+                for a in rows:
+                    self.readsA[a] += 1
+                self.readsB[b] += 1
+                retired = Bar(1)
 
-                        def mma(a=a, b=b, want_a=want_a, want_b=want_b, buf=buf, first=first, it=it):
-                            if self.slotA[a] != want_a:
-                                raise Violation(f"issuer {mi}: row slot {a} holds {self.slotA[a]}, expected {want_a}")
-                            if self.slotB[b] != want_b:
-                                raise Violation(f"issuer {mi}: weight slot {b} holds {self.slotB[b]}, expected {want_b}")
-                            acc = self.acc[buf]
-                            if acc['readers']:
-                                raise Violation(f"accumulator {buf} written for item {it} while the epilogue still reads item {acc['item']}")
-                            if acc['item'] != it:
-                                acc['item'], acc['done'] = it, 0
-                            acc['done'] += 1
-                            self.readsA[a] -= 1
-                            self.readsB[b] -= 1
-                        self.push(pipe, mma)
-                        self.push(pipe, self.emptyA[a].arrive)          # tcgen05.commit: after the MMAs above retire
-                        self.push(pipe, self.emptyB[b].arrive)
-                else:
-                    for jx in range(nst):
-                        yield (self.fullB[bs[jx]], bph[jx])
-                        self.emptyB[bs[jx]].arrive()                      # nothing of mine reads this weight tile
-                for _ in range(nst):
-                    a_slot += nsub
-                    if a_slot >= sa:
-                        a_slot, a_phase = a_slot - sa, a_phase ^ 1
-                    b_slot += 1
-                    if b_slot == sb:
-                        b_slot, b_phase = 0, b_phase ^ 1
-                t += nst
+                def group(rows=tuple(rows), b=b, it=it, t=t, acc=acc, retired=retired):
+                    for s_, a in enumerate(rows):
+                        if self.slotA[a] != (it, t, s_):
+                            raise Violation(f"consumer {g}: row slot {a} holds {self.slotA[a]}, expected {(it, t, s_)}")
+                    if self.slotB[b] != (it, t):
+                        raise Violation(f"consumer {g}: weight slot {b} holds {self.slotB[b]}, expected {(it, t)}")
+                    for a in rows:
+                        self.readsA[a] -= 1
+                    self.readsB[b] -= 1
+                    acc['done'] += len(rows)
+                    retired.arrive()
+                self.push(pipe, group)
+                if prev is not None:
+                    yield (prev[2], 0)                         # wgmma_wait<1>: the previous stage's group has retired
+                    for a in prev[0]:
+                        self.emptyA[a].arrive()
+                    self.emptyB[prev[1]].arrive()
+                prev = (rows, b, retired)
+                a_slot += nsub
+                if a_slot >= sa:
+                    a_slot, a_phase = a_slot - sa, a_phase ^ 1
+                b_slot += 1
+                if b_slot == sb:
+                    b_slot, b_phase = 0, b_phase ^ 1
                 yield None
-            if mine:
-                self.push(pipe, self.accFull[buf].arrive)
-            else:
-                self.accFull[buf].arrive()
-            n_item += 1
-            yield from self.layer_sync(f'issuer{mi}', it)
+            if prev is not None:
+                yield (prev[2], 0)                             # wgmma_wait<0>
+                for a in prev[0]:
+                    self.emptyA[a].arrive()
+                self.emptyB[prev[1]].arrive()
+            if acc['done'] != stages * nsub:
+                raise Violation(f"consumer {g}: epilogue of item {it} after {acc['done']} of {stages * nsub} sub-tile stages")
+            yield None                                         # epilogue: registers -> staging -> global
+            yield from self.layer_sync(f'consumer{g}', it)
 
     def gather(self, w):
         sa = self.sa
@@ -181,18 +169,18 @@ class Cta:
         for it, (nsub, stages) in enumerate(self.items):
             g_end = g_slot + stages * nsub
             while True:
-                if self.fixed_owners:                        # ring slot s is always filled by warp s % A_WARPS
+                if self.fixed_owners:                        # ring slot s is always filled by warp s % a_warps
                     if not (w < sa and p_lapb + p_sl < g_end):
                         break
                     sl, par, jl = p_sl, p_par, p_lapb + p_sl - g_slot
-                    p_sl += A_WARPS
+                    p_sl += self.a_warps
                     if p_sl >= sa:
                         p_sl, p_lapb, p_par = w, p_lapb + sa, p_par ^ 1
                 else:                                        # first version: slots dealt round-robin over the warps
                     if not nxt < g_end:
                         break
                     sl, par, jl = nxt % sa, (nxt // sa) & 1, nxt - g_slot
-                    nxt += A_WARPS
+                    nxt += self.a_warps
                 st, s = divmod(jl, nsub)
                 yield (self.emptyA[sl], par ^ 1)
                 bar, tag = self.fullA[sl], (it, st, s)
@@ -207,21 +195,6 @@ class Cta:
             g_slot = g_end
             yield from self.layer_sync(f'gather{w}', it)
 
-    def epilogue(self, q):
-        n_item = 0
-        for it, (nsub, stages) in enumerate(self.items):
-            buf = n_item & 1
-            yield (self.accFull[buf], (n_item >> 1) & 1)
-            acc = self.acc[buf]
-            if acc['item'] != it or acc['done'] != stages * nsub:
-                raise Violation(f"epilogue reads accumulator {buf} for item {it}: holds item {acc['item']} with {acc['done']} of {stages * nsub} MMAs")
-            acc['readers'] += 1
-            yield None                                        # TMEM loads, stores ...
-            acc['readers'] -= 1
-            self.accEmpty[buf].arrive()
-            n_item += 1
-            yield from self.layer_sync(f'epi{q}', it)
-
     def layer_sync(self, me, it):
         """__syncthreads() between the layers of a launch: every role waits for every other role here."""
         if it not in self.layer_ends:
@@ -232,9 +205,8 @@ class Cta:
 
     # ---- scheduler ---------------------------------------------------------------------------------
     def run(self):
-        roles = {'weights': self.weights(), 'issuer0': self.issuer(0), 'issuer1': self.issuer(1)}
-        roles.update({f'gather{w}': self.gather(w) for w in range(A_WARPS)})
-        roles.update({f'epi{q}': self.epilogue(q) for q in range(4)})
+        roles = {'weights': self.weights(), 'consumer0': self.consumer(0), 'consumer1': self.consumer(1)}
+        roles.update({f'gather{w}': self.gather(w) for w in range(self.a_warps)})
         blocked = {}                                          # role -> (bar, parity) | 'sync'
         steps = 0
         # late completions: with probability `lazy` an asynchronous agent is NOT offered to the scheduler in a round
@@ -288,8 +260,8 @@ def _items(rng, n, max_stages):
     return items, ends[:-1]
 
 
-# the ring shapes osb_conv_chain_launch builds: even row rings of 4..12 slots, 2 or 3 weight slots (up to CH_MAX_SB = 4);
-# the defaults are (10, 3) for N tiles up to 96 columns, (8, 3) for 128 and (8, 2) for 256
+# the ring shapes osb_conv_chain_launch builds: even row rings of 4..12 slots (4 = the least it accepts: two paired stages),
+# 2 to 4 weight slots; the defaults are (10, 3) for N tiles up to 96 columns and (8, 3) for 128
 RINGS = [(4, 2), (6, 3), (8, 2), (8, 3), (10, 3), (12, 3), (12, 2), (10, 4)]
 
 
@@ -303,21 +275,24 @@ def test_protocol_is_safe_and_live_under_random_schedules(sa, sb):
 
 def test_long_single_layer_many_laps():
     rng = random.Random(7)
-    Cta([(2, 81)] * 6 + [(1, 81)], 10, 3, rng).run()          # the level-0 96->96 layer: 27 offsets x 3 channel blocks per item
-    Cta([(1, 216)] * 3, 8, 2, rng).run()                      # a 256-wide N tile: single sub-tiles, 2 weight slots
+    Cta([(1, 81)] * 7, 10, 3, rng).run()                      # the level-0 96->96 layer: 27 offsets x 3 channel blocks per item
+    Cta([(2, 54)] * 6 + [(1, 54)], 10, 3, rng).run()          # a 64-wide N tile: paired sub-tiles
+    Cta([(1, 216)] * 3, 8, 3, rng).run()                      # a 128-wide N tile of a 256-channel layer
 
 
 def test_model_finds_the_round_robin_bug():
     """Negative control: slots dealt round-robin over the gather warps instead of fixed owners.  A warp then fills slot s on
     lap L and a DIFFERENT warp on lap L+1; nothing orders the two, and once there are at least as many gather warps as ring
     slots the later one can pass the parity test of `emptyA[s]` two phases early (phase L-2 looks like phase L) and overwrite
-    rows that were never multiplied -- the defect the first version of the kernel had.  The model must catch it; with fixed
-    owners the same ring is safe (RINGS above contains it)."""
+    rows that were never multiplied -- the defect the first version of the kernel had, with five gather warps on a ring of four
+    slots.  The model must catch it there; with fixed owners the same warps and ring are safe."""
     caught = 0
     for seed in range(60):
         rng = random.Random(seed)
         try:
-            Cta([(2, 27)] * 8, 4, 2, rng, fixed_owners=False).run()
+            Cta([(2, 27)] * 8, 4, 2, rng, fixed_owners=False, a_warps=5).run()
         except Violation:
             caught += 1
     assert caught >= 30, f"only {caught} of 60 schedules exposed the known defect"
+    for seed in range(20):
+        Cta([(2, 27)] * 8, 4, 2, random.Random(seed), fixed_owners=True, a_warps=5).run()

@@ -1,6 +1,6 @@
 """Persistent convolution chains (csrc/conv_chain.cu) against the fp64 oracle: every layer shape of the U-Net through a
-one-layer chain on grids of 148 and 3 CTAs (3 CTAs: every CTA walks many items -> sub-tile pairing, ring wrap-around, both
-TMEM buffers and both epilogue groups), forced split-K with the in-kernel reduction, the dense transposed form, and a
+one-layer chain on a grid of 148 CTAs requested (more than the SMs: the launcher clamps it to one CTA per SM) and of 3 CTAs
+(every CTA walks many items -> sub-tile pairing, ring wrap-around, both consumer warpgroups), forced split-K with the in-kernel reduction, the dense transposed form, and a
 BasicBlock chain (conv1 | downsample -> barrier -> conv2 + residual) in ONE launch.  Tolerance 1e-4 relative per row.
 Each configuration runs in its own process so that a trapped kernel cannot poison the CUDA context."""
 import os

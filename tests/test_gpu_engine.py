@@ -1,4 +1,4 @@
-"""Fused inference engine (tcgen05 path end to end) against the reference-topology golden activations and
+"""Fused inference engine (tensor-core path end to end) against the reference-topology golden activations and
 against the module-by-module surface.  Tolerance 1e-3 relative per point (north star); observed ~1e-5."""
 import numpy as np
 import pytest

@@ -1,113 +1,62 @@
-"""The CPU oracles against the REFERENCE's own functions, live, on random cases beyond the committed fixtures (build container
-only: needs /root/reference; the fixtures under tests/golden/ carry the same comparison to machines without the tree).
+"""The CPU oracles against what the REFERENCE's own functions returned on random cases beyond the original fixtures
+(tests/golden/live_*.npz, recorded by scripts/make_golden_live.py on the cases below).
 
 * oracle/fusion_ref.compute_mapping  vs  scripts/feature_fusion/fusion_util.py: PointCloudToImageMapper.compute_mapping
 * oracle/metric_ref                  vs  util/metric.py (confusion_matrix, evaluate) and util/util.py (intersectionAndUnion[GPU])
 Bit-exact (integer work); mIoU to 1e-12."""
-import os
-import sys
-import types
-
 import numpy as np
 import pytest
-import torch
 
-REF = os.environ.get('OSB_REFERENCE_ROOT', '/root/reference')
-needs_ref = pytest.mark.skipif(not os.path.exists(os.path.join(REF, 'util', 'metric.py')),
-                               reason='reference tree not present on this machine')
+from tests.util import digest, golden
 
 
-def _stub(*names):
-    made = []
-    for nm in names:
-        parts = nm.split('.')
-        for i in range(1, len(parts) + 1):
-            sub = '.'.join(parts[:i])
-            if sub not in sys.modules:
-                sys.modules[sub] = types.ModuleType(sub)
-                made.append(sub)
-            if i > 1:
-                setattr(sys.modules['.'.join(parts[:i - 1])], parts[i - 1], sys.modules[sub])
-    return made
-
-
-@pytest.fixture
-def ref_fusion_util():
-    made = _stub('tensorflow', 'tensorflow.io', 'tensorflow.compat', 'tensorflow.compat.v1')     # imported, never used by the mapper
-    path = os.path.join(REF, 'scripts', 'feature_fusion')
-    sys.path.insert(0, path)
-    sys.modules.pop('fusion_util', None)
-    try:
-        import fusion_util
-        yield fusion_util
-    finally:
-        sys.path.remove(path)
-        sys.modules.pop('fusion_util', None)
-        for m in made:
-            sys.modules.pop(m, None)
-
-
-@pytest.fixture
-def ref_metrics():
-    made = _stub('open3d', 'clip', 'matplotlib', 'matplotlib.patches', 'matplotlib.pyplot')
-    for name in [m for m in sys.modules if m == 'util' or m.startswith('util.') or m == 'dataset' or m.startswith('dataset.')]:
-        del sys.modules[name]
-    sys.path.insert(0, REF)
-    orig_cuda = torch.Tensor.cuda
-    torch.Tensor.cuda = lambda self, *a, **k: self           # intersectionAndUnionGPU calls .cuda(); no device here
-    try:
-        from util import metric as m, util as u
-        yield m, u
-    finally:
-        torch.Tensor.cuda = orig_cuda
-        sys.path.remove(REF)
-        for name in [m_ for m_ in sys.modules if m_ == 'util' or m_.startswith('util.') or m_ == 'dataset' or m_.startswith('dataset.')]:
-            del sys.modules[name]
-        for m_ in made:
-            sys.modules.pop(m_, None)
-
-
-@needs_ref
-def test_fusion_mapping_oracle_equals_the_reference_on_random_views(ref_fusion_util):
-    from oracle import fusion_ref
+def fusion_cases():
+    """[(seed, pts, poses, depths, intrinsics, cut_bound, visibility_threshold)] for seeds 100-107."""
     from openscene_b200.synth import fusion_case
-    n_vis = 0
+    out = []
     for seed in range(100, 108):
         with_depth = seed % 3 != 0
-        cut = [0, 5, 10, 20][seed % 4]
-        thres = [0.25, 0.1, 0.5][seed % 3]
         pts, poses, depths, intr = fusion_case(seed, 2500 + 300 * (seed % 5), with_depth)
-        mapper = ref_fusion_util.PointCloudToImageMapper(image_dim=(320, 240), intrinsics=intr, visibility_threshold=thres, cut_bound=cut)
-        for pose, depth in zip(poses, depths):
-            want = mapper.compute_mapping(pose, pts, depth)
-            got = fusion_ref.compute_mapping(pose, pts, depth, intr, (320, 240), cut, thres)
-            assert np.array_equal(got, want), seed
-            n_vis += int(want[:, 2].sum())
-    assert n_vis > 5000                                       # the cases exercise the visible branch
+        out.append((seed, pts, poses, depths, intr, [0, 5, 10, 20][seed % 4], [0.25, 0.1, 0.5][seed % 3]))
+    return out
 
 
-@needs_ref
-def test_metric_oracles_equal_the_reference_on_random_labels(ref_metrics):
-    from oracle import metric_ref
-    ref_metric, ref_util = ref_metrics
+def metric_cases():
+    """[(seed, n_classes, dataset name, pred, gt, has no-feature points)]: 15 % ignore labels, one class absent from gt."""
+    out = []
     for seed, (C, ds) in enumerate([(20, 'scannet_3d'), (21, 'matterport_3d'), (40, 'matterport_3d_40'), (80, 'matterport_3d_80'),
                                     (160, 'matterport_3d_160'), (16, 'nuscenes_3d')]):
         rng = np.random.RandomState(500 + seed)
         n = 20000
         gt = rng.randint(0, C, n)
         gt[rng.rand(n) < 0.15] = 255
-        gt[gt == (seed % C)] = (seed + 1) % C                  # one class never occurs in gt
+        gt[gt == (seed % C)] = (seed + 1) % C
         pred = np.where(rng.rand(n) < 0.5, np.minimum(gt, C - 1), rng.randint(0, C, n))
         nofeat = seed % 2 == 1
         if nofeat:
             pred[rng.rand(n) < 0.07] = 256
-        conf = ref_metric.confusion_matrix(pred.copy(), gt.copy(), C)
-        assert np.array_equal(metric_ref.confusion_matrix(pred, gt, C).astype(np.int64), conf.astype(np.int64)), ds
-        miou = ref_metric.evaluate(pred.copy(), gt.copy(), stdout=False, dataset=ds)
-        assert metric_ref.mean_iou(pred, gt, C)[0] == pytest.approx(float(miou), rel=1e-12), ds
+        out.append((seed, C, ds, pred, gt, nofeat))
+    return out
+
+
+def test_fusion_mapping_oracle_equals_the_reference_on_random_views():
+    from oracle import fusion_ref
+    g = golden('live_fusion_mapping.npz')
+    v = 0
+    for seed, pts, poses, depths, intr, cut, thres in fusion_cases():
+        for pose, depth in zip(poses, depths):
+            got = fusion_ref.compute_mapping(pose, pts, depth, intr, (320, 240), cut, thres)
+            assert digest(got) == g['maps'][v].decode(), seed
+            v += 1
+    assert v == len(g['maps']) and g['vis'].sum() > 5000                                       # the cases exercise the visible branch
+
+
+def test_metric_oracles_equal_the_reference_on_random_labels():
+    from oracle import metric_ref
+    g = golden('live_metric.npz')
+    for seed, C, ds, pred, gt, nofeat in metric_cases():
+        assert digest(metric_ref.confusion_matrix(pred, gt, C)) == g['conf'][seed].decode(), ds
+        assert metric_ref.mean_iou(pred, gt, C)[0] == pytest.approx(float(g['miou'][seed]), rel=1e-12), ds
         if not nofeat:
-            i_np, u_np, t_np = ref_util.intersectionAndUnion(pred.copy(), gt.copy(), C, 255)
-            i_t, u_t, t_t = ref_util.intersectionAndUnionGPU(torch.from_numpy(pred.copy()), torch.from_numpy(gt.copy()), C, 255)
-            i, u, t = metric_ref.intersection_and_union(pred, gt, C)
-            for a, b, c in ((i, i_np, i_t), (u, u_np, u_t), (t, t_np, t_t)):
-                assert np.array_equal(a, b.astype(np.int64)) and np.array_equal(a, c.numpy().astype(np.int64)), ds
+            for a, want in zip(metric_ref.intersection_and_union(pred, gt, C), g['iut'][seed]):
+                assert digest(a) == want.decode(), ds

