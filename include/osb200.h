@@ -221,6 +221,31 @@ int osb_conv_stem_fused(const float *in, int32_t cin, const int32_t *coords, int
                         int64_t cap, int32_t ks, int32_t step, const float *w, int32_t cout, const float *scale,
                         const float *shift, int32_t relu, void *out_split, float *out_f32, void *stream);
 
+/* Train-mode BatchNorm on split rows (`MinkowskiBatchNorm` / nn.BatchNorm1d with training=True over the [n, C] feature matrix;
+ * run/distill.py's validate() runs the network this way under no_grad).  The convolution before it runs with scale/shift =
+ * NULL and relu = 0; these two calls normalise its raw output.
+ *
+ * osb_bn_batch_stats: per-channel mean and biased variance over all n rows (every batch index together), then
+ *   scale = weight / sqrt(var + eps), shift = bias - mean * scale               (fp32 [c] outputs)
+ *   running_mean = (1 - m) running_mean + m mean, running_var = (1 - m) running_var + m var n / (n - 1),
+ *   num_batches_tracked += 1                                                   (in place, fp32 [c] / int64 [1])
+ * with m = momentum, or m = 1 / num_batches_tracked (after the increment) when momentum < 0 (momentum=None).  Values are
+ * accumulated in fp64 relative to the channel's value in row 0 (no E[x^2] - E[x]^2 cancellation); per-block partials are
+ * merged in a fixed order, so two calls give bit-identical results.  ws: osb_bn_stats_workspace_bytes(n, c) bytes (0 for
+ * shapes the call rejects).  Requires n >= 2 (as torch) and c a positive multiple of 32.
+ *
+ * osb_bn_apply_split: in place, x = act(x * scale + shift + r) with
+ *   r = 0                                    res_split == NULL
+ *   r = res                                  res_split given, res_scale == res_shift == NULL (BasicBlock identity shortcut)
+ *   r = res * res_scale + res_shift          all three given (the downsample branch's raw output with its own statistics)
+ *   act = max(., 0) when relu != 0.  res_split has the rows and channels of x and must not alias it. */
+size_t osb_bn_stats_workspace_bytes(int64_t n, int32_t c);
+int osb_bn_batch_stats(const void *x_split, int64_t n, int32_t c, const float *weight, const float *bias, double eps,
+                       double momentum, float *running_mean, float *running_var, int64_t *num_batches_tracked,
+                       float *scale, float *shift, void *ws, size_t ws_bytes, void *stream);
+int osb_bn_apply_split(void *x_split, int64_t n, int32_t c, const float *scale, const float *shift,
+                       const void *res_split, const float *res_scale, const float *res_shift, int32_t relu, void *stream);
+
 /* fp32 [n,c] <-> split rows. */
 int osb_f32_to_split(const float *in, int64_t n, int32_t c, void *out_split, void *stream);
 int osb_split_to_f32(const void *in_split, int64_t n, int32_t c, float *out, void *stream);

@@ -46,6 +46,9 @@ SIGNATURES = {
     'osb_conv_chain_launch': (c_int, [P, I32, P, I32, P]),
     'osb_tuning_set': (c_int, [c_char_p, I64]),
     'osb_conv_stem_fused': (c_int, [P, I32, P, I64, P, I64, I32, I32, P, I32, P, P, I32, P, P, P]),
+    'osb_bn_stats_workspace_bytes': (SZ, [I64, I32]),
+    'osb_bn_batch_stats': (c_int, [P, I64, I32, P, P, c_double, c_double, P, P, P, P, P, P, SZ, P]),
+    'osb_bn_apply_split': (c_int, [P, I64, I32, P, P, P, P, P, I32, P]),
     'osb_f32_to_split': (c_int, [P, I64, I32, P, P]),
     'osb_split_to_f32': (c_int, [P, I64, I32, P, P]),
     'osb_gather_rows_f32': (c_int, [P, P, I64, I32, P, P]),

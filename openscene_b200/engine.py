@@ -13,6 +13,13 @@ convolution:
 * the final 1x1x1 convolution writes fp32 rows straight into the caller's row order.
 
 Results equal the module-by-module path within the bf16x3 tolerance (tests/test_gpu_engine.py).
+
+``FusedMinkUNet(model, batch_stats=True)`` runs a TRAIN-mode network instead (the forward run/distill.py's validate() makes
+under no_grad): every BatchNorm normalises with the statistics of the current batch and moves its running buffers as
+``nn.BatchNorm1d`` does.  Each convolution then writes raw rows, ``osb_bn_batch_stats`` reduces them and
+``osb_bn_apply_split`` normalises them in place, with the ReLU and the BasicBlock residual (the downsample branch's raw output
+is normalised inside that same pass).  Layers run one launch each (a full reduction separates a layer from its consumer, so
+the persistent chain has nothing to fuse) (tests/test_gpu_bn_batch_stats.py).
 """
 import os
 
@@ -35,11 +42,11 @@ def _fold_bn(bn_module):
 
 
 class _Conv:
-    """Packed weights + folded BN of one convolution."""
+    """Packed weights + folded BN of one convolution (batch-statistics mode: the BatchNorm module instead, ``bn``)."""
     __slots__ = ('K', 'cin', 'cout', 'wpack', 'w3', 'scale', 'shift', 'ks', 'stride', 'transpose', 'wpack_a', 'scale_a', 'shift_a',
-                 'wtiles', 'wtiles_a', 'n_ntiles')
+                 'wtiles', 'wtiles_a', 'n_ntiles', 'bn', 'bs_args', 'bs_scale_a', 'bs_shift_a')
 
-    def __init__(self, conv, bn=None, keep_f32=False):
+    def __init__(self, conv, bn=None, keep_f32=False, fold=True):
         if getattr(conv, 'bias', None) is not None:
             raise NotImplementedError("FusedMinkUNet: convolutions with bias are not folded (no MinkUNet layer has one: "
                                       "models/mink_unet.py builds every convolution with bias=False)")
@@ -50,7 +57,8 @@ class _Conv:
         self.transpose = conv.TRANSPOSE
         self.w3 = w3.float().contiguous() if keep_f32 else None
         self.wpack = tc.pack_weights(w3) if (self.cin % 32 == 0 and self.cout % 32 == 0) else None
-        self.scale, self.shift = _fold_bn(bn) if bn is not None else (None, None)
+        self.scale, self.shift = _fold_bn(bn) if (bn is not None and fold) else (None, None)
+        self.bn = bn.bn if (bn is not None and not fold) else None
         # raw device addresses for the low-overhead launch path (tensors above keep the memory alive)
         self.wpack_a = self.wpack.data_ptr() if self.wpack is not None else 0
         self.wtiles = tc.pack_weight_tiles(w3) if self.wpack is not None else None        # persistent-kernel packing
@@ -61,19 +69,23 @@ class _Conv:
 
 
 class FusedMinkUNet:
-    def __init__(self, model):
-        """model: eval-mode MinkUNet (BasicBlock variants) whose parameters live on a CUDA device."""
+    def __init__(self, model, batch_stats=False):
+        """model: eval-mode MinkUNet (BasicBlock variants) whose parameters live on a CUDA device.
+        batch_stats=True: a train-mode model instead; every forward normalises with batch statistics and updates the BatchNorm
+        running buffers in place, as ``model(sinput)`` in train mode under no_grad does."""
         net = model.net3d if hasattr(model, 'net3d') else model
         p = next(net.parameters())
         C.require_cuda(p, 'model parameters')
-        if net.training:
-            raise RuntimeError("FusedMinkUNet folds BatchNorm running statistics: call model.eval() first")
+        self.batch_stats = bool(batch_stats)
+        self._net = net
+        self._check_mode()
         self.device = p.device
         self.dense_up = os.environ.get('OSB_DENSE_UP', '1') != '0'
         # The packed weights and folded BatchNorm constants are COPIES: every tensor they were made from is tracked, and a
-        # forward that finds one changed (load_state_dict, an optimiser step, .to()) re-packs before it runs.
-        self._net = net
-        self._tracked = list(net.parameters()) + list(net.buffers())
+        # forward that finds one changed (load_state_dict, an optimiser step, .to()) re-packs before it runs.  With batch
+        # statistics the running buffers are not copied (the kernels read and update the module's own), see _signature.
+        self._tracked = list(net.parameters()) + ([] if self.batch_stats else list(net.buffers()))
+        self._bs_ws = None
         self._build()
         self.out_channels = self.final.cout
         self.last_cm = None
@@ -89,32 +101,46 @@ class FusedMinkUNet:
         if 'OSB_TC_LAZY' in os.environ:                      # tuning: 0 = smem index prologue, 1 = lazy on >= 2-wave launches, 2 = always
             tc.debug_set_tc(lazy=int(os.environ['OSB_TC_LAZY']))
 
+    def _check_mode(self):
+        if self.batch_stats:
+            if not self._net.training or not all(m.training for m in self._net.modules()
+                                                 if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)):
+                raise RuntimeError("FusedMinkUNet(batch_stats=True) normalises with batch statistics (train-mode BatchNorm): "
+                                   "call model.train() first")
+        elif self._net.training:
+            raise RuntimeError("FusedMinkUNet folds BatchNorm running statistics: call model.eval() first")
+
     def _signature(self):
         # ~20 us for the 373 tensors of MinkUNet34C: in-place updates (optimiser steps, load_state_dict) bump `_version`; a
         # re-allocation (.to(), assign=True) moves the first / last tensor along with all others
         t = self._tracked
+        if self.batch_stats:
+            # weights and BatchNorm affine parameters by version; the running buffers only by address: the engine moves them
+            # itself every forward, which must not cost a re-pack, but a re-assigned buffer must be picked up
+            return (sum(x._version for x in t), tuple(x.data_ptr() for x in t),
+                    tuple(b.data_ptr() for m in self._bns for b in (m.running_mean, m.running_var, m.num_batches_tracked)))
         return (sum(x._version for x in t), t[0].data_ptr(), t[-1].data_ptr(), len(t))
 
     def refresh(self):
         """Re-pack the weights and re-fold BatchNorm from the source module (called automatically when a tracked tensor changed)."""
-        if self._net.training:
-            raise RuntimeError("FusedMinkUNet folds BatchNorm running statistics: call model.eval() first")
-        self._tracked = list(self._net.parameters()) + list(self._net.buffers())
+        self._check_mode()
+        self._tracked = list(self._net.parameters()) + ([] if self.batch_stats else list(self._net.buffers()))
         self._build()
 
     def _build(self):
         net = self._net
+        fold = not self.batch_stats
         with torch.cuda.device(self.device), torch.no_grad():
-            self.stem = _Conv(net.conv0p1s1, net.bn0, keep_f32=True)
+            self.stem = _Conv(net.conv0p1s1, net.bn0, keep_f32=True, fold=fold)
             if self.stem.cin > 3 or self.stem.cout != 32:
                 raise NotImplementedError("fused stem supports cin <= 3, cout == 32 (every MinkUNet: INIT_DIM = 32, 3 input features)")
             self.enc, self.dec = [], []
             for i in range(1, 5):
-                down = _Conv(getattr(net, f'conv{i}p{2 ** (i - 1)}s2'), getattr(net, f'bn{i}'))
-                self.enc.append((down, self._blocks(getattr(net, f'block{i}'))))
+                down = _Conv(getattr(net, f'conv{i}p{2 ** (i - 1)}s2'), getattr(net, f'bn{i}'), fold=fold)
+                self.enc.append((down, self._blocks(getattr(net, f'block{i}'), fold)))
             for j in range(4, 8):
                 m = getattr(net, f'convtr{j}p{2 ** (8 - j)}s2')
-                up = _Conv(m, getattr(net, f'bntr{j}'))
+                up = _Conv(m, getattr(net, f'bntr{j}'), fold=fold)
                 if self.dense_up and up.wpack is not None:
                     # dense transposed conv: one [cin, 8*cout] matrix, column block k = W[k]
                     wide = m.kernel.detach().permute(1, 0, 2).reshape(1, up.cin, up.K * up.cout).contiguous()
@@ -123,19 +149,70 @@ class FusedMinkUNet:
                     up.wtiles = tc.pack_weight_tiles(wide)
                     up.wtiles_a = up.wtiles.data_ptr()
                     up.n_ntiles = max(1, -(-(up.K * up.cout) // 128))
-                self.dec.append((up, self._blocks(getattr(net, f'block{j + 1}'))))
+                self.dec.append((up, self._blocks(getattr(net, f'block{j + 1}'), fold)))
             self.final = _Conv(net.final, None, keep_f32=True)
+            if self.batch_stats:
+                self._bs_setup()
         self._sig = self._signature()
 
     @staticmethod
-    def _blocks(seq):
+    def _blocks(seq, fold=True):
         out = []
         for b in seq:
             if not hasattr(b, 'conv2') or hasattr(b, 'conv3'):
                 raise NotImplementedError("FusedMinkUNet supports BasicBlock networks (all MinkUNet14/18/34 variants)")
-            ds = _Conv(b.downsample[0], b.downsample[1]) if b.downsample is not None else None
-            out.append((_Conv(b.conv1, b.norm1), _Conv(b.conv2, b.norm2), ds))
+            ds = _Conv(b.downsample[0], b.downsample[1], fold=fold) if b.downsample is not None else None
+            out.append((_Conv(b.conv1, b.norm1, fold=fold), _Conv(b.conv2, b.norm2, fold=fold), ds))
         return out
+
+    def _bs_setup(self):
+        """Batch-statistics mode: one engine-owned fp32 buffer holds the scale / shift of every BatchNorm (written by
+        osb_bn_batch_stats, read by osb_bn_apply_split); the kernels update the module's running buffers in place."""
+        convs = [self.stem]
+        for (c0, blocks) in self.enc + self.dec:
+            convs.append(c0)
+            convs += [cv for blk in blocks for cv in blk if cv is not None]
+        for cv in convs:
+            bn = cv.bn
+            if not (bn.affine and bn.track_running_stats):
+                raise NotImplementedError("FusedMinkUNet(batch_stats=True): BatchNorm without affine parameters or running "
+                                          "statistics is not supported (every MinkUNet BatchNorm has both)")
+            if (any(t.dtype != torch.float32 for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
+                    or bn.num_batches_tracked.dtype != torch.int64):
+                raise NotImplementedError("FusedMinkUNet(batch_stats=True): BatchNorm parameters and running statistics must be "
+                                          "fp32 (num_batches_tracked int64)")
+        self._bs_buf = torch.empty(sum(2 * cv.cout for cv in convs), dtype=torch.float32, device=self.device)
+        a = self._bs_buf.data_ptr()
+        for cv in convs:
+            bn = cv.bn
+            cv.bs_scale_a, cv.bs_shift_a = a, a + 4 * cv.cout
+            a += 8 * cv.cout
+            cv.bs_args = (bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                          bn.num_batches_tracked.data_ptr())
+        self._bns = [cv.bn for cv in convs]
+        self._bs_tensors = [t for m in self._bns for t in (m.running_mean, m.running_var, m.num_batches_tracked)]
+        self._bs_cmax = max(cv.cout for cv in convs)
+
+    def _bs_stats(self, cv, x_a, n):
+        """Batch statistics of cv's raw output rows: scale / shift into cv's slot, the module's running buffers moved."""
+        bn = cv.bn
+        w_a, b_a, rm_a, rv_a, nbt_a = cv.bs_args
+        rc = self._bs_stats_fn(x_a, n, cv.cout, w_a, b_a, bn.eps, -1.0 if bn.momentum is None else bn.momentum, rm_a, rv_a,
+                               nbt_a, cv.bs_scale_a, cv.bs_shift_a, self._bs_ws_a, self._bs_ws_bytes, self._stream)
+        if rc:
+            C.check(rc, 'osb_bn_batch_stats')
+
+    def _bs_apply(self, cv, x_a, n, relu=1, res_a=0, res_cv=None):
+        """x = act(x * scale + shift + r) in place; r = res, or the raw downsample output `res_a` normalised with res_cv's slot."""
+        rc = self._bs_apply_fn(x_a, n, cv.cout, cv.bs_scale_a, cv.bs_shift_a, res_a, res_cv.bs_scale_a if res_cv else 0,
+                               res_cv.bs_shift_a if res_cv else 0, relu, self._stream)
+        if rc:
+            C.check(rc, 'osb_bn_apply_split')
+
+    def _bs_norm(self, cv, x_a, n, relu=1, res_a=0, res_cv=None):
+        self._bs_stats(cv, x_a, n)
+        self._bs_apply(cv, x_a, n, relu, res_a, res_cv)
+        return x_a
 
     # ---------------------------------------------------------------------------------------
     # Launch path: activations of one forward live in ONE arena tensor; layers are addressed by raw
@@ -204,6 +281,8 @@ class FusedMinkUNet:
             self._chain.run(self._flags, self._stream)
 
     def _stage(self, blocks, srcs, nbr3_a, n):
+        if self.batch_stats:
+            return self._stage_bs(blocks, srcs, nbr3_a, n)
         x = srcs
         for (c1, c2, ds) in blocks:
             y = self._conv(c1, x, nbr3_a, n)
@@ -214,13 +293,46 @@ class FusedMinkUNet:
             x = [(self._conv(c2, [(y, c1.cout, n)], nbr3_a, n, res_a=r), c2.cout, n)]
         return x[0]
 
+    def _stage_bs(self, blocks, srcs, nbr3_a, n):
+        """BasicBlocks with batch statistics: raw convolutions, each normalised in place; the downsample branch is only reduced
+        (its normalisation happens inside conv2's apply pass, which reads it as the residual)."""
+        x = srcs
+        for (c1, c2, ds) in blocks:
+            y = self._bs_norm(c1, self._conv(c1, x, nbr3_a, n, relu=0), n)
+            if ds is not None:
+                r = self._conv(ds, x, 0, n, relu=0)
+                self._bs_stats(ds, r, n)
+            else:
+                r = x[0][0]
+            z = self._conv(c2, [(y, c1.cout, n)], nbr3_a, n, relu=0)
+            x = [(self._bs_norm(c2, z, n, res_a=r, res_cv=ds), c2.cout, n)]
+        return x[0]
+
     @torch.no_grad()
     def forward(self, coords, feats, coordinate_manager=None, head=None):
         """coords int32 [N,4] (batch,x,y,z), feats fp32 [N,cin], both CUDA, caller order.
-        Returns fp32 [N, out_channels] in the caller's row order (== ``model(SparseTensor(feats, coords))``)."""
+        Returns fp32 [N, out_channels] in the caller's row order (== ``model(SparseTensor(feats, coords))``).
+        batch_stats=True: == ``model(SparseTensor(feats, coords))`` in train mode, including the running-buffer updates."""
+        if not self.batch_stats:
+            return self._forward(coords, feats, coordinate_manager, head)
+        if head is not None:
+            raise NotImplementedError("FusedMinkUNet(batch_stats=True): the folded head is eval-only")
+        if not self._net.training or not all(m.training for m in self._bns):
+            self._check_mode()
+        self._bs_started = False
+        try:
+            return self._forward(coords, feats, coordinate_manager, None)
+        finally:
+            if self._bs_started:
+                # the kernels wrote the running buffers behind autograd's back: bump their versions as the module path's
+                # in-place updates do, so that an eval-mode engine or fast_eval on this model re-folds them
+                torch.autograd.graph.increment_version(self._bs_tensors)
+
+    def _forward(self, coords, feats, coordinate_manager, head):
         C.require_cuda(feats, 'features')
         if self._sig != self._signature():                     # the source module changed since the weights were packed
             self.refresh()
+        bs = self.batch_stats
         with torch.cuda.device(self.device):
             cm = coordinate_manager or CoordinateManager(coords, pyramid_levels=4 if self.use_pyramid else 0)
             self.last_cm = cm
@@ -228,6 +340,14 @@ class FusedMinkUNet:
             for _ in range(4):
                 ts_list.append(cm.stride(ts_list[-1], 2))
             n = [cm.sets[t].n for t in ts_list]
+            if bs:
+                # level sizes are known here: refuse before anything is launched, so that no running buffer moves
+                for l in range(5):
+                    if n[l] < 2:
+                        c = self.stem.cout if l == 0 else self.enc[l - 1][0].cout
+                        raise ValueError(f"Expected more than 1 value per channel when training, got input size [{n[l]}, {c}] "
+                                         f"(level {l}, tensor stride {ts_list[l]})")
+                self._bs_started = True
             nbr3 = [cm.kernel_map(t, t, 3).nbr for t in ts_list]
             down = [cm.kernel_map(ts_list[l], ts_list[l + 1], 2) for l in range(4)]
             up_nbr = [d.transposed().nbr for d in down] if not self.dense_up else None
@@ -246,7 +366,16 @@ class FusedMinkUNet:
             self._ws_a, self._ws_bytes = self._ws.data_ptr(), self._ws.numel()
             self._stream = torch.cuda.current_stream().cuda_stream
             self._fn = C.lib().osb_conv_fwd_tc
-            self._chain_on = self.use_chain
+            self._chain_on = self.use_chain and not bs           # batch statistics: one launch per layer (see module doc)
+            if bs:
+                # statistics workspace: grow-only like the arena; one suffices, the reductions run one after another in the stream
+                ws_q = C.lib().osb_bn_stats_workspace_bytes
+                need_bs = max(ws_q(nl, self._bs_cmax) for nl in n)
+                if self._bs_ws is None or self._bs_ws.numel() < need_bs:
+                    self._bs_ws = None
+                    self._bs_ws = torch.empty(max(need_bs, 256), dtype=torch.uint8, device=self.device)
+                self._bs_ws_a, self._bs_ws_bytes = self._bs_ws.data_ptr(), self._bs_ws.numel()
+                self._bs_stats_fn, self._bs_apply_fn = C.lib().osb_bn_batch_stats, C.lib().osb_bn_apply_split
             if self._chain_on:
                 if self._chain is None:
                     self._chain = tc.ConvChain(self.device, 160)
@@ -267,16 +396,21 @@ class FusedMinkUNet:
             st = self.stem
             x_a = self._cursor
             self._cursor += _al(n[0] * 4 * st.cout)
+            relu = 0 if bs else 1                           # batch statistics: raw convolutions (scale_a / shift_a are 0)
             if cs0.grid is not None:
                 C.call('osb_conv_stem_fused_grid', C.ptr(x_int), st.cin, C.ptr(cs0.coords), n[0], C.ptr(cs0.grid), *cs0.grid_args,
-                       st.ks, 1, C.ptr(st.w3), st.cout, st.scale_a, st.shift_a, 1, x_a, None, self._stream)
+                       st.ks, 1, C.ptr(st.w3), st.cout, st.scale_a, st.shift_a, relu, x_a, None, self._stream)
             else:
                 C.call('osb_conv_stem_fused', C.ptr(x_int), st.cin, C.ptr(cs0.coords), n[0], C.ptr(cs0.slots), cs0.cap, st.ks, 1,
-                       C.ptr(st.w3), st.cout, st.scale_a, st.shift_a, 1, x_a, None, self._stream)
+                       C.ptr(st.w3), st.cout, st.scale_a, st.shift_a, relu, x_a, None, self._stream)
+            if bs:
+                self._bs_norm(st, x_a, n[0])
             skips = [(x_a, st.cout, n[0])]
             cur = skips[0]
             for l, (dconv, blocks) in enumerate(self.enc):
-                y = self._conv(dconv, [cur], down[l].nbr.data_ptr(), n[l + 1])
+                y = self._conv(dconv, [cur], down[l].nbr.data_ptr(), n[l + 1], relu=relu)
+                if bs:
+                    self._bs_norm(dconv, y, n[l + 1])
                 cur = self._stage(blocks, [(y, dconv.cout, n[l + 1])], nbr3_a[l + 1], n[l + 1])
                 skips.append(cur)
             for j, (uconv, blocks) in enumerate(self.dec):
@@ -292,11 +426,13 @@ class FusedMinkUNet:
                     if self.layer_log is not None:
                         self.layer_log.append((n[l + 1], 1, cur[1], uconv.K * uconv.cout, 'dense-up'))
                     rc = C.lib().osb_convtr_fwd_tc(cur[0], cur[1], n[l + 1], down[l].nbr.data_ptr(), uconv.K, uconv.wpack_a,
-                                                   uconv.cout, uconv.scale_a, uconv.shift_a, 1, y, 0, self._flags, self._stream)
+                                                   uconv.cout, uconv.scale_a, uconv.shift_a, relu, y, 0, self._flags, self._stream)
                     if rc:
                         C.check(rc, 'osb_convtr_fwd_tc')
                 else:
-                    y = self._conv(uconv, [cur], up_nbr[l].data_ptr(), n[l])
+                    y = self._conv(uconv, [cur], up_nbr[l].data_ptr(), n[l], relu=relu)
+                if bs:
+                    self._bs_norm(uconv, y, n[l])
                 cur = self._stage(blocks, [(y, uconv.cout, n[l]), skips[l]], nbr3_a[l], n[l])
             if head is not None:                           # folded head: 96 -> (96 + K) conv, rows straight in caller order
                 z = torch.empty((n[0], head.cout), dtype=torch.float32, device=self.device)
@@ -325,6 +461,8 @@ class FusedMinkUNet:
     def fold_head(self, text_features):
         """Pre-compute the folded head for a set of unit-norm text embeddings [K, C_out]:
         W W^T = L L^T (Cholesky, fp64) and U = W T^T, packed as one 1x1x1 convolution 96 -> (96 + K)."""
+        if self.batch_stats:
+            raise NotImplementedError("fold_head: the folded head is eval-only (FusedMinkUNet without batch_stats)")
         W = self.final.w3[0].double()                                    # [cin, cout]
         T = text_features.to(W.device).double()                          # [K, cout]
         G = W @ W.t()
@@ -350,6 +488,8 @@ class FusedMinkUNet:
         """Cosine scores / labels of every voxel against the folded text set (``fold_head``), equal to
         ``match(normalize(forward(coords, feats)), text)`` up to rounding, without the 768-d features.
         Returns (scores fp16 [N,K] or None, label int64 [N], smax fp32 [N]) in the caller's row order."""
+        if self.batch_stats:
+            raise NotImplementedError("forward_scores: the folded head is eval-only (FusedMinkUNet without batch_stats)")
         cv, cin, k = folded[:3]
         if len(folded) > 3 and folded[3] != self._signature():
             raise RuntimeError("forward_scores: the folded head was built from weights that have changed since; call fold_head again")
