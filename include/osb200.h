@@ -246,6 +246,33 @@ int osb_bn_batch_stats(const void *x_split, int64_t n, int32_t c, const float *w
 int osb_bn_apply_split(void *x_split, int64_t n, int32_t c, const float *scale, const float *shift,
                        const void *res_split, const float *res_scale, const float *res_shift, int32_t relu, void *stream);
 
+/* Training (FusedMinkUNet.forward_train, openscene_b200/engine_train.py; run/distill.py's training step).  The forward keeps what the backward needs:
+ *
+ * osb_bn_batch_stats_save: osb_bn_batch_stats that also writes the batch mean and invstd = 1 / sqrt(var + eps) (fp32 [c]).
+ *   The backward needs them; they cannot be recovered from scale / shift when weight == 0.
+ * osb_bn_apply_split_out: osb_bn_apply_split into separate output rows y_split (x_split, the raw convolution output z, is
+ *   kept for the backward).  y_split must not overlap x_split or res_split.
+ *
+ * Backward of y = act(BN(z) + r) given the incoming gradient g (all split rows [n, c]):
+ *   g' = g [y > 0] (y_split given: the ReLU mask), or g' = g (y_split NULL: no activation), x^ = (z - mean) invstd
+ * osb_bn_backward_reduce: sums = (sum g', sum g' x^) (fp32 [2, c]); dbias = sum g', dweight = sum g' x^ (fp32 [c]),
+ *   overwritten, or added to the buffers' values when accumulate != 0.  Sums are taken in fp64 and per-block partials
+ *   merged in a fixed order (bit-reproducible, no atomics).  ws: osb_bn_stats_workspace_bytes(n, c) bytes.
+ * osb_bn_backward_apply: dz = weight invstd (g' - sums[0] / n - x^ sums[1] / n) into dz_split, with the sums of
+ *   osb_bn_backward_reduce.  gp_split (may be NULL) receives g' (gp_accumulate == 0) or gp_split += g': the gradient of the
+ *   BasicBlock's identity shortcut.  dz_split and gp_split must not overlap each other or y, g, z. */
+int osb_bn_batch_stats_save(const void *x_split, int64_t n, int32_t c, const float *weight, const float *bias, double eps,
+                            double momentum, float *running_mean, float *running_var, int64_t *num_batches_tracked,
+                            float *scale, float *shift, float *mean, float *invstd, void *ws, size_t ws_bytes, void *stream);
+int osb_bn_apply_split_out(const void *x_split, void *y_split, int64_t n, int32_t c, const float *scale, const float *shift,
+                           const void *res_split, const float *res_scale, const float *res_shift, int32_t relu, void *stream);
+int osb_bn_backward_reduce(const void *y_split, const void *g_split, const void *z_split, int64_t n, int32_t c,
+                           const float *mean, const float *invstd, float *sums, float *dweight, float *dbias,
+                           int32_t accumulate, void *ws, size_t ws_bytes, void *stream);
+int osb_bn_backward_apply(const void *y_split, const void *g_split, const void *z_split, int64_t n, int32_t c,
+                          const float *mean, const float *invstd, const float *weight, const float *sums, void *dz_split,
+                          void *gp_split, int32_t gp_accumulate, void *stream);
+
 /* fp32 [n,c] <-> split rows. */
 int osb_f32_to_split(const float *in, int64_t n, int32_t c, void *out_split, void *stream);
 int osb_split_to_f32(const void *in_split, int64_t n, int32_t c, float *out, void *stream);

@@ -49,6 +49,10 @@ SIGNATURES = {
     'osb_bn_stats_workspace_bytes': (SZ, [I64, I32]),
     'osb_bn_batch_stats': (c_int, [P, I64, I32, P, P, c_double, c_double, P, P, P, P, P, P, SZ, P]),
     'osb_bn_apply_split': (c_int, [P, I64, I32, P, P, P, P, P, I32, P]),
+    'osb_bn_batch_stats_save': (c_int, [P, I64, I32, P, P, c_double, c_double, P, P, P, P, P, P, P, P, SZ, P]),
+    'osb_bn_apply_split_out': (c_int, [P, P, I64, I32, P, P, P, P, P, I32, P]),
+    'osb_bn_backward_reduce': (c_int, [P, P, P, I64, I32, P, P, P, P, P, I32, P, SZ, P]),
+    'osb_bn_backward_apply': (c_int, [P, P, P, I64, I32, P, P, P, P, P, P, I32, P]),
     'osb_f32_to_split': (c_int, [P, I64, I32, P, P]),
     'osb_split_to_f32': (c_int, [P, I64, I32, P, P]),
     'osb_gather_rows_f32': (c_int, [P, P, I64, I32, P, P]),

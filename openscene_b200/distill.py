@@ -90,6 +90,25 @@ def distill_step(model, optimizer, coords, feats, feat_3d, mask, loss_type='cosi
     return loss.detach()
 
 
+def fused_distill_step(engine, optimizer, coords, feats, feat_3d, mask, loss_type='cosine', translate=True):
+    """``distill_step`` on the fused engine: the same random translation, loss, zero_grad, backward and optimiser step, with
+    the forward and backward of ``engine.forward_train(..., rows=mask)`` (a ``FusedMinkUNet(model, batch_stats=True)``).
+    Single process only: DistributedDataParallel wraps ``model.forward``, which the engine bypasses."""
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise RuntimeError("fused_distill_step: the fused engine does not all-reduce gradients (world size > 1); "
+                           "use distill_step on the DistributedDataParallel model")
+    if translate:
+        coords = coords.clone()
+        coords[:, 1:4] += (torch.rand(3) * 100).type_as(coords)
+    dev = engine.device
+    out = engine.forward_train(coords.to(dev, non_blocking=True), feats.to(dev, non_blocking=True), rows=mask.to(dev))
+    loss = distill_loss(out, feat_3d.to(dev), loss_type)
+    optimizer.zero_grad()
+    loss.backward()
+    optimizer.step()
+    return loss.detach()
+
+
 def wrap_ddp(model, device=None):
     if dist.is_initialized() and dist.get_world_size() > 1:
         ids = [device.index] if device is not None and device.type == 'cuda' else None

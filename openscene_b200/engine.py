@@ -44,7 +44,8 @@ def _fold_bn(bn_module):
 class _Conv:
     """Packed weights + folded BN of one convolution (batch-statistics mode: the BatchNorm module instead, ``bn``)."""
     __slots__ = ('K', 'cin', 'cout', 'wpack', 'w3', 'scale', 'shift', 'ks', 'stride', 'transpose', 'wpack_a', 'scale_a', 'shift_a',
-                 'wtiles', 'wtiles_a', 'n_ntiles', 'bn', 'bs_args', 'bs_scale_a', 'bs_shift_a')
+                 'wtiles', 'wtiles_a', 'n_ntiles', 'bn', 'bs_args', 'bs_scale_a', 'bs_shift_a', 'mod', 'bs_mean_a', 'bs_invstd_a',
+                 'bwd')
 
     def __init__(self, conv, bn=None, keep_f32=False, fold=True):
         if getattr(conv, 'bias', None) is not None:
@@ -55,6 +56,7 @@ class _Conv:
         self.K, self.cin, self.cout = w3.shape
         self.ks, self.stride = conv.kernel_size, conv.stride
         self.transpose = conv.TRANSPOSE
+        self.mod, self.bwd = conv, None          # training: the module (parameter -> gradient slot), W^T packs for dgrad
         self.w3 = w3.float().contiguous() if keep_f32 else None
         self.wpack = tc.pack_weights(w3) if (self.cin % 32 == 0 and self.cout % 32 == 0) else None
         self.scale, self.shift = _fold_bn(bn) if (bn is not None and fold) else (None, None)
@@ -86,6 +88,8 @@ class FusedMinkUNet:
         # statistics the running buffers are not copied (the kernels read and update the module's own), see _signature.
         self._tracked = list(net.parameters()) + ([] if self.batch_stats else list(net.buffers()))
         self._bs_ws = None
+        self._gen = 0                             # bumped by every forward: a training graph whose activations were overwritten
+        self._garena = []                         # training: grow-only chunks of gradient rows (engine_train.py)
         self._build()
         self.out_channels = self.final.cout
         self.last_cm = None
@@ -181,12 +185,14 @@ class FusedMinkUNet:
                     or bn.num_batches_tracked.dtype != torch.int64):
                 raise NotImplementedError("FusedMinkUNet(batch_stats=True): BatchNorm parameters and running statistics must be "
                                           "fp32 (num_batches_tracked int64)")
-        self._bs_buf = torch.empty(sum(2 * cv.cout for cv in convs), dtype=torch.float32, device=self.device)
+        # per BatchNorm: scale, shift and (forward_train) the batch mean / invstd the backward reads
+        self._bs_buf = torch.empty(sum(4 * cv.cout for cv in convs), dtype=torch.float32, device=self.device)
         a = self._bs_buf.data_ptr()
         for cv in convs:
             bn = cv.bn
             cv.bs_scale_a, cv.bs_shift_a = a, a + 4 * cv.cout
-            a += 8 * cv.cout
+            cv.bs_mean_a, cv.bs_invstd_a = a + 8 * cv.cout, a + 12 * cv.cout
+            a += 16 * cv.cout
             cv.bs_args = (bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
                           bn.num_batches_tracked.data_ptr())
         self._bns = [cv.bn for cv in convs]
@@ -348,6 +354,7 @@ class FusedMinkUNet:
                         raise ValueError(f"Expected more than 1 value per channel when training, got input size [{n[l]}, {c}] "
                                          f"(level {l}, tensor stride {ts_list[l]})")
                 self._bs_started = True
+            self._gen += 1
             nbr3 = [cm.kernel_map(t, t, 3).nbr for t in ts_list]
             down = [cm.kernel_map(ts_list[l], ts_list[l + 1], 2) for l in range(4)]
             up_nbr = [d.transposed().nbr for d in down] if not self.dense_up else None
@@ -456,6 +463,14 @@ class FusedMinkUNet:
             return ext
 
     __call__ = forward
+
+    def forward_train(self, coords, feats, rows=None):
+        """Training forward of a batch_stats engine with a device backward (openscene_b200/engine_train.py).
+        Returns fp32 rows with a grad_fn: ``model(SparseTensor(feats, coords))`` (rows=None, caller order) or its ``[rows]``
+        (bool mask or int64 caller-row index; only those rows go through the final 1x1x1 layer).  ``loss.backward()`` then
+        writes / accumulates ``.grad`` of every parameter of the model.  The running buffers move once per call."""
+        from . import engine_train
+        return engine_train.forward_train(self, coords, feats, rows)
 
     # ---------------------------------------------------------------------------------------
     def fold_head(self, text_features):
