@@ -273,6 +273,31 @@ int osb_bn_backward_apply(const void *y_split, const void *g_split, const void *
                           const float *mean, const float *invstd, const float *weight, const float *sums, void *dz_split,
                           void *gp_split, int32_t gp_accumulate, void *stream);
 
+/* Softmax cross-entropy head (FusedMinkUNet.forward_train_ce, openscene_b200/engine_train.py; run/train_mink.py's step):
+ * the final 1x1x1 convolution cin -> C of a per-voxel classifier, `CrossEntropyLoss(ignore_index)` over its rows (mean over
+ * the labelled rows) and `output.max(1)[1]`, without writing the logits.
+ *   x_split      the network's last activation, split rows [n, cin] in internal order; cin a multiple of 32 up to 384
+ *   w            fp32 [cin, C], 1 <= C <= 160
+ *   row_map      int32 [n]: caller row of internal row r (the coordinate manager's perm, a permutation of 0..n-1);
+ *                labels are read and pred written in caller order through it
+ *   labels       int32 or int64 [n] (labels_are_i64), caller order; a label outside [0, C) other than ignore_index makes the
+ *                loss NaN (callers validate labels first); labels are only read at row_map[r]
+ *   ws           osb_ce_head_workspace_bytes(n, cin, C) bytes, 256-byte aligned (0 for shapes the calls reject)
+ * osb_ce_head_fwd: z = x w (fp32 accumulation), lse[r] = log sum exp z (fp32 [n], internal order), pred[row_map[r]] = first
+ *   argmax of z (int64), n_valid = number of rows whose label != ignore_index (int64 [1]), loss (fp32 [1]) = sum over those
+ *   rows of lse - z[label] / n_valid, NaN when n_valid == 0.  The sum is fp64 with per-block partials merged in a fixed order.
+ * osb_ce_head_bwd: with g (fp32 [1], the upstream gradient of loss) and n_valid read on the device (no host sync):
+ *   d = (softmax(z) - onehot(label)) g / n_valid on labelled rows, 0 elsewhere (z recomputed, softmax = exp(z - lse));
+ *   dx_split = d w^T (split rows [n, cin], internal order), dw = sum_r x_r^T d_r (fp32 [cin, C], overwritten).  Every
+ *   output is exactly 0 when n_valid == 0.  Partials are merged in a fixed order: two calls give identical bits. */
+size_t osb_ce_head_workspace_bytes(int64_t n, int32_t cin, int32_t C);
+int osb_ce_head_fwd(const void *x_split, int64_t n, int32_t cin, const float *w, int32_t C, const int32_t *row_map,
+                    const void *labels, int32_t labels_are_i64, int64_t ignore_index, float *lse, int64_t *pred, float *loss,
+                    int64_t *n_valid, void *ws, size_t ws_bytes, void *stream);
+int osb_ce_head_bwd(const void *x_split, int64_t n, int32_t cin, const float *w, int32_t C, const int32_t *row_map,
+                    const void *labels, int32_t labels_are_i64, int64_t ignore_index, const float *lse, const float *g,
+                    const int64_t *n_valid, void *dx_split, float *dw, void *ws, size_t ws_bytes, void *stream);
+
 /* fp32 [n,c] <-> split rows. */
 int osb_f32_to_split(const float *in, int64_t n, int32_t c, void *out_split, void *stream);
 int osb_split_to_f32(const void *in_split, int64_t n, int32_t c, float *out, void *stream);

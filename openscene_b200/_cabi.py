@@ -53,6 +53,9 @@ SIGNATURES = {
     'osb_bn_apply_split_out': (c_int, [P, P, I64, I32, P, P, P, P, P, I32, P]),
     'osb_bn_backward_reduce': (c_int, [P, P, P, I64, I32, P, P, P, P, P, I32, P, SZ, P]),
     'osb_bn_backward_apply': (c_int, [P, P, P, I64, I32, P, P, P, P, P, P, I32, P]),
+    'osb_ce_head_workspace_bytes': (SZ, [I64, I32, I32]),
+    'osb_ce_head_fwd': (c_int, [P, I64, I32, P, I32, P, P, I32, I64, P, P, P, P, P, SZ, P]),
+    'osb_ce_head_bwd': (c_int, [P, I64, I32, P, I32, P, P, I32, I64, P, P, P, P, P, P, SZ, P]),
     'osb_f32_to_split': (c_int, [P, I64, I32, P, P]),
     'osb_split_to_f32': (c_int, [P, I64, I32, P, P]),
     'osb_gather_rows_f32': (c_int, [P, P, I64, I32, P, P]),

@@ -90,6 +90,7 @@ class FusedMinkUNet:
         self._bs_ws = None
         self._gen = 0                             # bumped by every forward: a training graph whose activations were overwritten
         self._garena = []                         # training: grow-only chunks of gradient rows (engine_train.py)
+        self._ce_ws = None                        # training: workspace of the cross-entropy head (engine_train.py)
         self._build()
         self.out_channels = self.final.cout
         self.last_cm = None
@@ -471,6 +472,15 @@ class FusedMinkUNet:
         writes / accumulates ``.grad`` of every parameter of the model.  The running buffers move once per call."""
         from . import engine_train
         return engine_train.forward_train(self, coords, feats, rows)
+
+    def forward_train_ce(self, coords, feats, labels, ignore_index=-100):
+        """Training step of a per-voxel classifier on a batch_stats engine (run/train_mink.py): returns ``(loss, pred)`` with
+        ``loss == F.cross_entropy(model(SparseTensor(feats, coords)), labels, ignore_index=ignore_index)`` (0-dim fp32 with a
+        grad_fn) and ``pred == output.max(1)[1]`` (int64 [N], caller order, up to ties).  Any head of 1 to 160 classes on a
+        trunk of width a multiple of 32 up to 384.  ``loss.backward()`` fills ``.grad`` of every parameter; the logits are
+        never materialised (openscene_b200/engine_train.py, csrc/ce_head.cu)."""
+        from . import engine_train
+        return engine_train.forward_train_ce(self, coords, feats, labels, ignore_index)
 
     # ---------------------------------------------------------------------------------------
     def fold_head(self, text_features):

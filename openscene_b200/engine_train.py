@@ -15,7 +15,11 @@ Backward, in reverse layer order, everything in split rows:
   * the stem: wgrad only, ``osb_conv_wgrad_tc`` over the 5^3 map with the 3 input channels zero-padded to 32 (the input
     features get no gradient).
 A tensor with several consumers collects its gradient in a fixed order through the ``res`` operand of the dgrad (output and
-residual never alias), so two identical steps give bit-identical gradients."""
+residual never alias), so two identical steps give bit-identical gradients.
+
+``forward_train_ce`` (per-voxel classification, run/train_mink.py) runs the same trunk and replaces the final layer by
+``osb_ce_head_fwd`` (head product, log-sum-exp, NLL over the labelled rows, argmax in caller order); its backward starts with
+``osb_ce_head_bwd``, which writes the head's weight gradient and the trunk output's gradient, and continues as above."""
 import torch
 from torch.autograd.function import once_differentiable
 
@@ -72,10 +76,107 @@ def forward_train(eng, coords, feats, rows=None):
     if eng._sig != eng._signature():                     # weights changed (optimiser step): re-pack before anything runs
         eng.refresh()
     if eng.final.wpack is None:
-        raise NotImplementedError("forward_train: the final layer's widths must be multiples of 32 (tensor-core head)")
+        raise NotImplementedError("forward_train: the final layer's widths must be multiples of 32 (tensor-core head); "
+                                  "a classifier head with cross-entropy trains through forward_train_ce")
     _ensure_bwd_packs(eng)
     params = list(eng._net.parameters())
     return _TrainFunction.apply(eng, coords, feats, rows, *params)
+
+
+CE_MAX_CLASSES = 160
+CE_CIN = (32, 64, 96, 128, 160, 192, 224, 256, 288, 320, 352, 384)
+
+
+def forward_train_ce(eng, coords, feats, labels, ignore_index=-100):
+    """(loss, pred): ``F.cross_entropy(model(SparseTensor(feats, coords)), labels, ignore_index=ignore_index)`` with a grad_fn,
+    and ``output.max(1)[1]`` (int64, caller order).  The trunk runs as in forward_train; the final 1x1x1 layer, the loss and
+    the argmax are one launch (osb_ce_head_fwd) and its backward another (osb_ce_head_bwd): the logits never exist."""
+    _refuse(eng, feats)
+    C.require_cuda(feats, 'features')
+    if not isinstance(labels, torch.Tensor) or labels.dtype == torch.bool or labels.is_floating_point() or labels.is_complex():
+        raise TypeError(f"forward_train_ce: labels must be an integer tensor (got {getattr(labels, 'dtype', type(labels))})")
+    if labels.dim() != 1 or labels.shape[0] != feats.shape[0]:
+        raise ValueError(f"forward_train_ce: labels of shape {tuple(labels.shape)} for {feats.shape[0]} rows (expected [N])")
+    if eng._sig != eng._signature():
+        eng.refresh()
+    fin = eng.final
+    if fin.cout > CE_MAX_CLASSES or fin.cin not in CE_CIN or fin.K != 1:
+        raise NotImplementedError(f"forward_train_ce: a 1x1x1 head of {fin.cin} -> {fin.cout} channels (supported: input width a "
+                                  f"multiple of 32 up to 384, 1 to {CE_MAX_CLASSES} classes)")
+    labels = labels.to(eng.device)
+    if labels.dtype not in (torch.int32, torch.int64):
+        labels = labels.long()
+    labels = labels.contiguous()
+    ignore_index = int(ignore_index)
+    bad = (labels != ignore_index) & ((labels < 0) | (labels >= fin.cout))
+    if bool(bad.any()):                                 # before anything is launched: no running buffer moves
+        raise IndexError(f"forward_train_ce: Target {int(labels[bad][0])} is out of bounds for {fin.cout} classes")
+    _ensure_bwd_packs(eng)
+    params = list(eng._net.parameters())
+    return _CEFunction.apply(eng, coords, feats, labels, ignore_index, *params)
+
+
+def _ce_workspace(eng, n, cin, c):
+    need = C.lib().osb_ce_head_workspace_bytes(n, cin, c)
+    if eng._ce_ws is None or eng._ce_ws.numel() < need:
+        eng._ce_ws = None
+        eng._ce_ws = torch.empty(max(need, 256), dtype=torch.uint8, device=eng.device)
+    return eng._ce_ws.data_ptr(), eng._ce_ws.numel()
+
+
+def _ce_forward(eng, cm, cur, n0, ce, tape):
+    """osb_ce_head_fwd on the trunk's last activation; records what the backward reads"""
+    labels, ignore = ce
+    fin, dev = eng.final, eng.device
+    lse = torch.empty(n0, dtype=torch.float32, device=dev)
+    pred = torch.empty(n0, dtype=torch.int64, device=dev)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    n_valid = torch.empty(1, dtype=torch.int64, device=dev)
+    ws_a, ws_b = _ce_workspace(eng, n0, cur[1], fin.cout)
+    i64 = 1 if labels.dtype == torch.int64 else 0
+    rc = C.lib().osb_ce_head_fwd(cur[0], n0, cur[1], fin.w3.data_ptr(), fin.cout, cm.perm.data_ptr(), labels.data_ptr(), i64,
+                                 ignore, lse.data_ptr(), pred.data_ptr(), loss.data_ptr(), n_valid.data_ptr(), ws_a, ws_b,
+                                 eng._stream)
+    if rc:
+        C.check(rc, 'osb_ce_head_fwd')
+    tape.append(('ce_head', (_Node(fin, 0, 0, n0, [cur], 1, 0, 0), cm.perm, labels, ignore, lse, n_valid)))
+    return loss, pred
+
+
+def _ce_backward(eng, item, g, slot, galloc, grads, stream):
+    """osb_ce_head_bwd: dW into the final kernel's gradient slot, dx = the gradient of the trunk's last activation"""
+    nd, perm, labels, ignore, lse, n_valid = item
+    cv = nd.cv
+    (src, c, n0), = nd.srcs
+    dx = galloc(n0 * 4 * c)
+    ws_a, ws_b = _ce_workspace(eng, n0, c, cv.cout)
+    i64 = 1 if labels.dtype == torch.int64 else 0
+    rc = C.lib().osb_ce_head_bwd(src, n0, c, cv.w3.data_ptr(), cv.cout, perm.data_ptr(), labels.data_ptr(), i64, ignore,
+                                 lse.data_ptr(), g.data_ptr(), n_valid.data_ptr(), dx, slot(cv.mod.kernel).data_ptr(), ws_a, ws_b,
+                                 stream)
+    if rc:
+        C.check(rc, 'osb_ce_head_bwd')
+    grads[src] = dx
+
+
+class _CEFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, eng, coords, feats, labels, ignore, *params):
+        graph = _run_forward(eng, coords, feats, None, ce=(labels, ignore))
+        loss, pred = graph.out
+        graph.out = None
+        ctx.eng, ctx.graph = eng, graph
+        ctx.save_for_backward(*params)
+        ctx.mark_non_differentiable(pred)
+        return loss, pred
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g, _g_pred):
+        params = ctx.saved_tensors
+        grads = _run_backward(ctx.eng, ctx.graph, g, params)
+        ctx.graph = None
+        return (None, None, None, None, None) + tuple(grads)
 
 
 def _ensure_bwd_packs(eng):
@@ -141,7 +242,7 @@ class _TrainFunction(torch.autograd.Function):
         return (None, None, None, None) + tuple(grads)
 
 
-def _run_forward(eng, coords, feats, rows):
+def _run_forward(eng, coords, feats, rows, ce=None):
     dev = eng.device
     st = eng.stem
     with torch.cuda.device(dev):
@@ -155,7 +256,7 @@ def _run_forward(eng, coords, feats, rows):
                 c = st.cout if l == 0 else eng.enc[l - 1][0].cout
                 raise ValueError(f"Expected more than 1 value per channel when training, got input size [{n[l]}, {c}] "
                                  f"(level {l}, tensor stride {ts[l]})")
-        sel = _select(cm, rows, n[0], dev)
+        sel = _select(cm, rows, n[0], dev) if ce is None else None
         eng._gen += 1                                    # from here on the arena is overwritten
         eng.last_cm = cm
         m3 = [cm.kernel_map(t, t, 3) for t in ts]
@@ -163,9 +264,11 @@ def _run_forward(eng, coords, feats, rows):
         # every map the backward reads is built now, before the first launch of the step
         nbr3 = [(k.nbr.data_ptr(), k.transposed().nbr.data_ptr()) for k in m3]
         dn = [(d.nbr.data_ptr(), d.transposed().nbr.data_ptr()) for d in down]
-        m = sel.shape[0]
-        sel_t = torch.empty(n[0], dtype=torch.int32, device=dev)
-        C.call('osb_kernel_map_transpose', C.ptr(sel), m, 1, C.ptr(sel_t), n[0], C.stream_ptr())
+        m, sel_t = n[0], None
+        if ce is None:
+            m = sel.shape[0]
+            sel_t = torch.empty(n[0], dtype=torch.int32, device=dev)
+            C.call('osb_kernel_map_transpose', C.ptr(sel), m, 1, C.ptr(sel_t), n[0], C.stream_ptr())
         k5 = cm.kernel_map(1, 1, st.ks)
 
         need = plan_train_bytes(eng, n) + 256
@@ -275,12 +378,15 @@ def _run_forward(eng, coords, feats, rows):
         if eng._cursor > end:
             raise RuntimeError("forward_train: activation arena overflow (plan_train_bytes out of date)")
         fin = eng.final
-        out = torch.empty((m, fin.cout), dtype=torch.float32, device=dev)
-        rc = eng._fn(cur[0], cur[1], n[0], 0, 0, 0, sel.data_ptr(), m, 1, fin.wpack_a, fin.cout, 0, 0, 0, 0, 0, out.data_ptr(), 0,
-                     eng._ws_a, eng._ws_bytes, eng._flags, eng._stream)
-        if rc:
-            C.check(rc, 'osb_conv_fwd_tc')
-        tape.append(('head', _Node(fin, 0, 0, n[0], [cur], 1, sel.data_ptr(), sel_t.data_ptr())))
+        if ce is None:
+            out = torch.empty((m, fin.cout), dtype=torch.float32, device=dev)
+            rc = eng._fn(cur[0], cur[1], n[0], 0, 0, 0, sel.data_ptr(), m, 1, fin.wpack_a, fin.cout, 0, 0, 0, 0, 0, out.data_ptr(),
+                         0, eng._ws_a, eng._ws_bytes, eng._flags, eng._stream)
+            if rc:
+                C.check(rc, 'osb_conv_fwd_tc')
+            tape.append(('head', _Node(fin, 0, 0, n[0], [cur], 1, sel.data_ptr(), sel_t.data_ptr())))
+        else:
+            out = _ce_forward(eng, cm, cur, n[0], ce, tape)
         if eng.layer_log is not None:
             eng.layer_log.append((m, 1, cur[1], fin.cout, 'head'))
     torch.autograd.graph.increment_version(eng._bs_tensors)
@@ -408,6 +514,8 @@ def _run_backward(eng, gr, g, params):
                 if rc:
                     C.check(rc, 'osb_conv_fwd_tc')
                 grads[src] = out
+            elif kind == 'ce_head':
+                _ce_backward(eng, item, g, slot, galloc, grads, stream)
             elif kind == 'block':
                 n1, nd_, n2 = item
                 g2 = grads[n2.y]
