@@ -323,6 +323,27 @@ int osb_match_ensemble(const float *feat3d, const void *feat2d_f16, int64_t n_vo
                        const void *text_f16, int32_t k_text, void *scores_f16, int64_t *label, void *feat_out_f16,
                        void *stream);
 
+/* Test-time repeat vote (run/evaluate.py:385-425 with test_repeats > 1).  The product of osb_match_scores /
+ * osb_match_ensemble (same arguments, same fp16 scores s), and in the same pass, for every point p and column k:
+ *   store[p,k] = fp16_rn(store[p,k] + s[p,k])          in/out fp16 [n_pts, K], zero before the first repeat
+ *   label_cur[p] = argmax_k s[p,k],  label_acc[p] = argmax_k store[p,k]  (int64, may be NULL)
+ * The argmax is torch's CPU `x.float().max(1)[1]`: the first NaN of a row if it holds one, else the first maximum.
+ * scores_f16 (may be NULL) receives s bit-identical to osb_match_scores; otherwise s never reaches memory.
+ * 1 <= K <= 480.  Store bits are the reference's `store = pred + store` on the CPU applied in repeat order. */
+int osb_match_vote(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c, const int64_t *inds_reverse,
+                   int64_t n_pts, const void *text_f16, int32_t k_text, int32_t normalize, void *scores_f16,
+                   void *store_f16, int64_t *label_cur, int64_t *label_acc, void *stream);
+int osb_match_ensemble_vote(const float *feat3d, const void *feat2d_f16, int64_t n_vox, int32_t c,
+                            const int64_t *inds_reverse, int64_t n_pts, const float *smax3d, const float *smax2d,
+                            const void *text_f16, int32_t k_text, void *scores_f16, void *store_f16, int64_t *label_cur,
+                            int64_t *label_acc, void *stream);
+/* The same vote from a score or logit matrix already in memory (run/eval_mink.py:193-212):
+ *   store[p,k] += src[v,k]   v = inds_reverse[p] (or p when NULL, then n_src == n_pts), in the source's precision
+ *                            (src_is_f16: fp16 source and store, one fp16 add rounded to nearest even; else fp32)
+ *   label_cur / label_acc as above.  1 <= K <= 512. */
+int osb_vote_accumulate(const void *src, int32_t src_is_f16, int64_t n_src, const int64_t *inds_reverse, int64_t n_pts,
+                        int32_t k, void *store, int64_t *label_cur, int64_t *label_acc, void *stream);
+
 /* Optional folded head (engine.forward_scores): rows z = [x L | x U] (fp32, row pitch ld floats) from one 1x1x1
  * convolution with the weights [L | U], W W^T = L L^T, U = W T^T  ->  score_k = fp16((x.U_k) / (|x L| + 1e-5)),
  * label = first argmax.  Same cosine scores as run/evaluate.py:305-310 without materialising the 768-d features. */

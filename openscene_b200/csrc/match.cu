@@ -135,6 +135,13 @@ int match_tc_run(const void *feat, int feat_is_f16, const void *feat2_f16, const
                  const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize,
                  void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, cudaStream_t stream);
 
+int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
+                      const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize,
+                      void *scores_f16, void *store_f16, int64_t *label_cur, int64_t *label_acc, cudaStream_t stream);
+// CUDA-core repeat vote (vote.cu)
+int vote_accumulate_run(const void *src, int src_is_f16, const int64_t *inds_reverse, int64_t n_pts, int k, void *store,
+                        int64_t *label_cur, int64_t *label_acc, cudaStream_t stream);
+
 static bool use_simt() {   // OSB_MATCH_SIMT=1 selects the CUDA-core kernels below (cross-check path)
   static int v = -1;
   if (v < 0) { const char *e = getenv("OSB_MATCH_SIMT"); v = (e && e[0] == '1') ? 1 : 0; }
@@ -199,6 +206,57 @@ int osb_match_ensemble(const float *feat3d, const void *feat2d_f16, int64_t n_vo
                                                   (__half *)feat_out_f16);
   OSB_LAUNCH_CHECK();
   return 0;
+}
+
+// Repeat vote.  The tensor-core path adds the fp16 scores into the store in the epilogue of the product (the scores reach
+// HBM only when asked for); OSB_MATCH_SIMT=1 writes them to a scratch buffer with the CUDA-core kernels above and votes
+// with k_vote_accumulate.  Both give the same bits.
+static int match_vote_simt(int rc, void *scratch, bool own, int64_t n_pts, int32_t k_text, void *store_f16,
+                           int64_t *label_cur, int64_t *label_acc, cudaStream_t stream) {
+  if (rc == 0) rc = vote_accumulate_run(scratch, 1, nullptr, n_pts, k_text, store_f16, label_cur, label_acc, stream);
+  if (own) cudaFreeAsync(scratch, stream);
+  return rc;
+}
+
+static int check_vote_args(const char *fn, int32_t c, int32_t k_text, int64_t n_vox, int64_t n_pts, const void *store_f16) {
+  OSB_CHECK(c == 512 || c == 768, "%s: feature width %d unsupported (OpenScene uses 512 / 768)", fn, c);
+  OSB_CHECK(k_text >= 1 && k_text <= 480, "%s: K_text=%d outside 1..480", fn, k_text);
+  OSB_CHECK(n_vox > 0 && n_pts >= 0, "%s: bad shape", fn);
+  OSB_CHECK(store_f16 != nullptr, "%s: null store", fn);
+  return 0;
+}
+
+int osb_match_vote(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c, const int64_t *inds_reverse,
+                   int64_t n_pts, const void *text_f16, int32_t k_text, int32_t normalize, void *scores_f16,
+                   void *store_f16, int64_t *label_cur, int64_t *label_acc, void *stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (check_vote_args("osb_match_vote", c, k_text, n_vox, n_pts, store_f16)) return 1;
+  if (n_pts == 0) return 0;
+  if (!use_simt())
+    return match_tc_vote_run(feat, feat_is_f16, nullptr, nullptr, nullptr, c, inds_reverse, n_pts, text_f16, k_text,
+                             normalize, scores_f16, store_f16, label_cur, label_acc, stream);
+  void *scratch = scores_f16;
+  if (scratch == nullptr) OSB_CUDA(cudaMallocAsync(&scratch, (size_t)n_pts * k_text * sizeof(__half), stream));
+  const int rc = osb_match_scores(feat, feat_is_f16, n_vox, c, inds_reverse, n_pts, text_f16, k_text, normalize, scratch,
+                                  nullptr, nullptr, stream_);
+  return match_vote_simt(rc, scratch, scores_f16 == nullptr, n_pts, k_text, store_f16, label_cur, label_acc, stream);
+}
+
+int osb_match_ensemble_vote(const float *feat3d, const void *feat2d_f16, int64_t n_vox, int32_t c,
+                            const int64_t *inds_reverse, int64_t n_pts, const float *smax3d, const float *smax2d,
+                            const void *text_f16, int32_t k_text, void *scores_f16, void *store_f16, int64_t *label_cur,
+                            int64_t *label_acc, void *stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (check_vote_args("osb_match_ensemble_vote", c, k_text, n_vox, n_pts, store_f16)) return 1;
+  if (n_pts == 0) return 0;
+  if (!use_simt())
+    return match_tc_vote_run(feat3d, 0, feat2d_f16, smax3d, smax2d, c, inds_reverse, n_pts, text_f16, k_text, 0,
+                             scores_f16, store_f16, label_cur, label_acc, stream);
+  void *scratch = scores_f16;
+  if (scratch == nullptr) OSB_CUDA(cudaMallocAsync(&scratch, (size_t)n_pts * k_text * sizeof(__half), stream));
+  const int rc = osb_match_ensemble(feat3d, feat2d_f16, n_vox, c, inds_reverse, n_pts, smax3d, smax2d, text_f16, k_text,
+                                    scratch, nullptr, nullptr, stream_);
+  return match_vote_simt(rc, scratch, scores_f16 == nullptr, n_pts, k_text, store_f16, label_cur, label_acc, stream);
 }
 
 }  // extern "C"

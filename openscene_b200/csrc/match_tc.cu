@@ -13,7 +13,12 @@
 // TMA (rows >= K_text are out of bounds -> zero fill).  Warps 0-7 (two warpgroups, 64 points each) then run `wgmma` f16
 // (M=64, N=96 per pass, K=16) into register accumulators, round to fp16, keep the first-maximum argmax over the passes and
 // write scores / labels / row maxima.  HBM-bound: 4*C (or 2*C) bytes per point against 2*C*K flops.
+//
+// k_match_tc_vote is the same kernel with the test-time repeat vote in the epilogue: each fp16 score is added into the
+// caller's fp16 store in place and the labels of the score row and of the summed row are kept (vote.cuh), so a repeat's
+// [N_pts, K] scores never reach HBM.  k_match_tc itself compiles to the same instructions as before the vote existed.
 #include "tc_ptx.cuh"
+#include "vote.cuh"
 #include <algorithm>
 
 namespace osb {
@@ -38,9 +43,17 @@ struct MatchTcParams {
   __half *feat_out;                  // [n_pts, C] or NULL: the fp16 operand actually multiplied (ensemble feature)
 };
 
-template <int NP>   // half2 pairs per lane: C = 64 * NP
-__global__ void __launch_bounds__(MT_THREADS, 1)
-k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
+// Test-time repeat vote (k_match_tc_vote): store[p,k] = fp16_rn(store[p,k] + scores[p,k]) in place, and the labels of
+// this repeat's scores and of the accumulated sum (vote.cuh: torch CPU `max(1)[1]`, NaN-first).
+struct MatchTcVote {
+  __half *store;                     // [n_pts, k_text]
+  int64_t *label_cur;                // [n_pts] or NULL
+  int64_t *label_acc;                // [n_pts] or NULL
+  int pair;                          // K even and the store 4-byte aligned: a thread's column pair is one __half2
+};
+
+template <int NP, bool VOTE>   // half2 pairs per lane: C = 64 * NP
+__device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const MatchTcParams p, const MatchTcVote vo) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int C = 64 * NP;
@@ -163,6 +176,8 @@ k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
     const int cq = 2 * (lane & 3);
     float best[2] = {-INFINITY, -INFINITY};
     int best_k[2] = {0, 0};
+    VoteArgmax vcur[2], vacc[2];
+    if constexpr (VOTE) { vcur[0].init(); vcur[1].init(); vacc[0].init(); vacc[1].init(); }
     mbar_wait(a_full, 0);
     int s = 0; uint32_t phase = 0;
     for (int pass = 0; pass < p.n_pass; ++pass) {
@@ -188,44 +203,113 @@ k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
       for (int h = 0; h < 2; ++h) {
         const int64_t pt = row0 + r_lo + 8 * h;
 #pragma unroll
-        for (int i = 0; i < MT_NW / 8; ++i)
+        for (int i = 0; i < MT_NW / 8; ++i) {
+          if constexpr (VOTE) {
+            // the thread's two adjacent columns k0, k0 + 1 of this row (k0 even): one 4-byte store access when the pair is
+            // aligned (vo.pair), two 2-byte accesses otherwise
+            const int k0 = pass * MT_NW + 8 * i + cq;
+            if (k0 < p.k_text) {
+              const bool two = k0 + 1 < p.k_text;
+              const __half h0 = __float2half_rn(acc[4 * i + 2 * h]);
+              const __half h1 = __float2half_rn(acc[4 * i + 2 * h + 1]);
+              if (p.scores != nullptr && pt < p.n_pts) {
+                p.scores[pt * p.k_text + k0] = h0;
+                if (two) p.scores[pt * p.k_text + k0 + 1] = h1;
+              }
+              vcur[h].take(__half2float(h0), k0);
+              if (two) vcur[h].take(__half2float(h1), k0 + 1);
+              if (pt < p.n_pts) {
+                __half *st = vo.store + pt * p.k_text + k0;
+                __half s0, s1;
+                if (two && vo.pair) {
+                  // one fp16 add per lane, round to nearest even
+                  const __half2 sum = __hadd2(*reinterpret_cast<const __half2 *>(st), __halves2half2(h0, h1));
+                  *reinterpret_cast<__half2 *>(st) = sum;
+                  s0 = __low2half(sum);
+                  s1 = __high2half(sum);
+                } else {
+                  s0 = __hadd(st[0], h0);
+                  st[0] = s0;
+                  s1 = s0;
+                  if (two) { s1 = __hadd(st[1], h1); st[1] = s1; }
+                }
+                vacc[h].take(__half2float(s0), k0);
+                if (two) vacc[h].take(__half2float(s1), k0 + 1);
+              }
+            }
+          } else {
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int k = pass * MT_NW + 8 * i + cq + e;       // ascending per thread: the first maximum is kept
-            if (k < p.k_text) {
-              const __half hv = __float2half_rn(acc[4 * i + 2 * h + e]);
-              const float sc = __half2float(hv);
-              if (p.scores != nullptr && pt < p.n_pts) p.scores[pt * p.k_text + k] = hv;
-              if (sc > best[h]) { best[h] = sc; best_k[h] = k; }
+            for (int e = 0; e < 2; ++e) {
+              const int k = pass * MT_NW + 8 * i + cq + e;       // ascending per thread: the first maximum is kept
+              if (k < p.k_text) {
+                const __half hv = __float2half_rn(acc[4 * i + 2 * h + e]);
+                const float sc = __half2float(hv);
+                if (p.scores != nullptr && pt < p.n_pts) p.scores[pt * p.k_text + k] = hv;
+                if (sc > best[h]) { best[h] = sc; best_k[h] = k; }
+              }
             }
           }
+        }
       }
     }
-    // the four lanes of a row hold interleaved column pairs: the maximum with the smallest column wins
+    if constexpr (VOTE) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-      for (int o = 1; o < 4; o <<= 1) {
-        const float ob = __shfl_xor_sync(0xffffffffu, best[h], o);
-        const int ok = __shfl_xor_sync(0xffffffffu, best_k[h], o);
-        if (ob > best[h] || (ob == best[h] && ok < best_k[h])) { best[h] = ob; best_k[h] = ok; }
+      for (int h = 0; h < 2; ++h) {
+        vcur[h].reduce<4>();
+        vacc[h].reduce<4>();
+        const int64_t pt = row0 + r_lo + 8 * h;
+        if ((lane & 3) == 0 && pt < p.n_pts) {
+          if (vo.label_cur) vo.label_cur[pt] = vcur[h].k;
+          if (vo.label_acc) vo.label_acc[pt] = vacc[h].k;
+        }
       }
-      const int64_t pt = row0 + r_lo + 8 * h;
-      if ((lane & 3) == 0 && pt < p.n_pts) {
-        if (p.label) p.label[pt] = best_k[h];
-        if (p.smax) p.smax[pt] = best[h];
+    } else {
+      // the four lanes of a row hold interleaved column pairs: the maximum with the smallest column wins
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {
+          const float ob = __shfl_xor_sync(0xffffffffu, best[h], o);
+          const int ok = __shfl_xor_sync(0xffffffffu, best_k[h], o);
+          if (ob > best[h] || (ob == best[h] && ok < best_k[h])) { best[h] = ob; best_k[h] = ok; }
+        }
+        const int64_t pt = row0 + r_lo + 8 * h;
+        if ((lane & 3) == 0 && pt < p.n_pts) {
+          if (p.label) p.label[pt] = best_k[h];
+          if (p.smax) p.smax[pt] = best[h];
+        }
       }
     }
   }
 }
 
-static int launch_match_tc(const MatchTcParams &p, const void *text_f16, cudaStream_t stream) {
+template <int NP>
+__global__ void __launch_bounds__(MT_THREADS, 1)
+k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
+  match_tc_body<NP, false>(tmT, p, MatchTcVote{});
+}
+
+template <int NP>
+__global__ void __launch_bounds__(MT_THREADS, 1)
+k_match_tc_vote(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, const MatchTcVote vo) {
+  match_tc_body<NP, true>(tmT, p, vo);
+}
+
+static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, const void *text_f16, cudaStream_t stream) {
   CUtensorMap tmT;
   if (make_tmap_2b(&tmT, text_f16, (uint64_t)p.C, (uint64_t)p.k_text, MT_NW, 1)) return 1;
   const int NP = p.C / 64;
   const size_t smem = (size_t)NP * MT_M * 128 + MT_BSTAGES * MT_NW * 128 + 128 + 1024;
   const unsigned grid = (unsigned)ceil_div(p.n_pts, MT_M);
-  if (NP == 12) {
+  if (vote != nullptr) {
+    if (NP == 12) {
+      OSB_SMEM_ATTR_ONCE(k_match_tc_vote<12>, 227 * 1024);
+      k_match_tc_vote<12><<<grid, MT_THREADS, smem, stream>>>(tmT, p, *vote);
+    } else {
+      OSB_SMEM_ATTR_ONCE(k_match_tc_vote<8>, 227 * 1024);
+      k_match_tc_vote<8><<<grid, MT_THREADS, smem, stream>>>(tmT, p, *vote);
+    }
+  } else if (NP == 12) {
     OSB_SMEM_ATTR_ONCE(k_match_tc<12>, 227 * 1024);
     k_match_tc<12><<<grid, MT_THREADS, smem, stream>>>(tmT, p);
   } else {
@@ -236,17 +320,39 @@ static int launch_match_tc(const MatchTcParams &p, const void *text_f16, cudaStr
   return 0;
 }
 
-int match_tc_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
-                 const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize,
-                 void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, cudaStream_t stream) {
-  MatchTcParams p{};
+static int fill_match_tc(MatchTcParams &p, const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a,
+                         const float *sel_b, int c, const int64_t *inds_reverse, int64_t n_pts, int k_text, int normalize,
+                         void *scores_f16, int64_t *label, float *smax, void *feat_out_f16) {
+  p = MatchTcParams{};
   p.feat = feat; p.feat2 = (const __half *)feat2_f16; p.sel_a = sel_a; p.sel_b = sel_b;
   p.inds_reverse = inds_reverse; p.n_pts = n_pts; p.C = c; p.k_text = k_text;
   p.n_pass = (k_text + MT_NW - 1) / MT_NW;
   OSB_CHECK(p.n_pass * MT_NW <= 512, "match: K_text=%d too large (at most 512 text rows)", k_text);
   p.feat_is_f16 = feat_is_f16; p.normalize = normalize;
   p.scores = (__half *)scores_f16; p.label = label; p.smax = smax; p.feat_out = (__half *)feat_out_f16;
-  return launch_match_tc(p, text_f16, stream);
+  return 0;
+}
+
+int match_tc_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
+                 const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize,
+                 void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, cudaStream_t stream) {
+  MatchTcParams p;
+  if (fill_match_tc(p, feat, feat_is_f16, feat2_f16, sel_a, sel_b, c, inds_reverse, n_pts, k_text, normalize, scores_f16,
+                    label, smax, feat_out_f16))
+    return 1;
+  return launch_match_tc(p, nullptr, text_f16, stream);
+}
+
+int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
+                      const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize,
+                      void *scores_f16, void *store_f16, int64_t *label_cur, int64_t *label_acc, cudaStream_t stream) {
+  MatchTcParams p;
+  if (fill_match_tc(p, feat, feat_is_f16, feat2_f16, sel_a, sel_b, c, inds_reverse, n_pts, k_text, normalize, scores_f16,
+                    nullptr, nullptr, nullptr))
+    return 1;
+  const MatchTcVote vote{(__half *)store_f16, label_cur, label_acc,
+                         (k_text % 2 == 0 && reinterpret_cast<uintptr_t>(store_f16) % 4 == 0) ? 1 : 0};
+  return launch_match_tc(p, &vote, text_f16, stream);
 }
 
 }  // namespace osb

@@ -90,12 +90,17 @@ def evaluate(pred_ids, gt_ids, stdout=False, dataset='scannet_3d'):
     m.update(pred_ids, gt_ids)
     mean_iou, mean_acc, ious = m.evaluate()
     if stdout:
-        print('evaluating', int(torch.as_tensor(gt_ids).numel()), 'points...')
-        for i, v in ious.items():
-            print('class {0:<4d}: {1:>5.3f}   ({2:>6d}/{3:<6d})'.format(i, v[0], int(v[1]), int(v[2])))
-        print('Mean IoU', mean_iou)
-        print('Mean Acc', mean_acc)
+        print_evaluation(int(torch.as_tensor(gt_ids).numel()), mean_iou, mean_acc, ious)
     return mean_iou
+
+
+def print_evaluation(n_points, mean_iou, mean_acc, ious):
+    """The report ``evaluate(..., stdout=True)`` prints (util/metric.py:80-101)."""
+    print('evaluating', n_points, 'points...')
+    for i, v in ious.items():
+        print('class {0:<4d}: {1:>5.3f}   ({2:>6d}/{3:<6d})'.format(i, v[0], int(v[1]), int(v[2])))
+    print('Mean IoU', mean_iou)
+    print('Mean Acc', mean_acc)
 
 
 def intersectionAndUnionGPU(output, target, K, ignore_index=255):
