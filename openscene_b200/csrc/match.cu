@@ -3,7 +3,12 @@
 // [N_pts, C].  Replaces the torch ops at run/evaluate.py:288-323.
 //
 // HBM-bound: 4*C bytes read per point (3 KB at C = 768) against 2*C*K flops; one warp owns one
-// point, the text matrix (K*C*2 bytes, <= 245 KB) stays in L1/L2.
+// point, the text matrix (K*C*2 bytes, <= 737 KB at K = 480) stays in L1/L2.
+//
+// Label rule of every non-vote kernel (k_match_scores, k_match_ensemble, k_match_tc, k_folded_head_finish): the lowest
+// column holding the largest non-NaN score, and 0 when no score is above -inf (a row of NaN and -inf only); smax is that
+// largest non-NaN score, -inf when there is none.  Labels always lie in [0, K).  torch's CUDA `max(1)[1]`, which the
+// reference takes, returns a NaN's index instead; the repeat vote follows torch's CPU rule (vote.cuh).
 #include "common.cuh"
 #include <algorithm>
 #include <stdlib.h>
@@ -163,7 +168,8 @@ int osb_match_scores(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32
                      int64_t *label, float *smax, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(c == 512 || c == 768, "osb_match_scores: feature width %d unsupported (OpenScene uses 512 / 768)", c);
-  OSB_CHECK(k_text >= 1 && n_vox > 0, "osb_match_scores: bad shape");
+  OSB_CHECK(k_text >= 1 && k_text <= 480, "osb_match_scores: K_text=%d outside 1..480", k_text);
+  OSB_CHECK(n_vox > 0, "osb_match_scores: bad shape");
   if (n_pts == 0) return 0;
   if (!use_simt())
     return match_tc_run(feat, feat_is_f16, nullptr, nullptr, nullptr, c, inds_reverse, n_pts, text_f16, k_text, normalize,
@@ -190,7 +196,8 @@ int osb_match_ensemble(const float *feat3d, const void *feat2d_f16, int64_t n_vo
                        void *scores_f16, int64_t *label, void *feat_out_f16, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(c == 512 || c == 768, "osb_match_ensemble: feature width %d unsupported", c);
-  OSB_CHECK(k_text >= 1 && n_vox > 0, "osb_match_ensemble: bad shape");
+  OSB_CHECK(k_text >= 1 && k_text <= 480, "osb_match_ensemble: K_text=%d outside 1..480", k_text);
+  OSB_CHECK(n_vox > 0, "osb_match_ensemble: bad shape");
   if (n_pts == 0) return 0;
   if (!use_simt())
     return match_tc_run(feat3d, 0, feat2d_f16, smax3d, smax2d, c, inds_reverse, n_pts, text_f16, k_text, 0, scores_f16, label,
@@ -281,7 +288,7 @@ __global__ void k_folded_head_finish(const float *__restrict__ z, int64_t n, int
     for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
     const float d = sqrtf(ss) + 1e-5f;
     float best = -INFINITY;
-    int best_k = 0x7fffffff;
+    int best_k = 0;          // the label rule above: 0 when no score is above -inf
     for (int k = lane; k < k_text; k += 32) {
       const __half h = __float2half_rn(__ldg(row + c_norm + k) / d);
       if (scores) scores[p * k_text + k] = h;

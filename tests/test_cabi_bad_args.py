@@ -56,3 +56,34 @@ def test_degenerate_arguments_fail_with_a_message_and_never_crash():
     for name in ('osb_conv_chain_workspace_bytes', 'osb_conv_tc_workspace_bytes', 'osb_conv_wgrad_tc_workspace_bytes',
                  'osb_conv_packed_weight_bytes', 'osb_conv_weight_tiles_bytes', 'osb_occgrid_bytes'):
         assert res[name + ':null'][0] == 0 and res[name + ':neg'][0] == 0, name
+
+
+_K_CHILD = r'''
+import json, sys
+sys.path.insert(0, sys.argv[1])
+from openscene_b200 import _cabi as C
+L = C.lib()
+out = {}
+def run(name, *args):
+    return [getattr(L, name)(*args), (L.osb_last_error() or b'').decode()]
+for k in (0, -1, 481, 512, 100000):
+    # valid widths and counts, NULL buffers: only the text count is wrong, and it must be refused before any launch
+    out['osb_match_scores:%d' % k] = run('osb_match_scores', None, 0, 10, 768, None, 10, None, k, 0, None, None, None, None)
+    out['osb_match_ensemble:%d' % k] = run('osb_match_ensemble', None, None, 10, 512, None, 10, None, None, None, k, None,
+                                           None, None, None)
+    out['osb_match_vote:%d' % k] = run('osb_match_vote', None, 0, 10, 768, None, 10, None, k, 0, None, None, None, None,
+                                       None)
+print('RESULT ' + json.dumps(out))
+'''
+
+
+def test_match_entry_points_refuse_text_counts_outside_1_to_480_on_both_routes():
+    """the tensor-core kernel streams at most five 96-row passes; both routes refuse any other K on the host"""
+    for simt in ('0', '1'):
+        p = subprocess.run([sys.executable, '-c', _K_CHILD, ROOT], capture_output=True, text=True, timeout=300,
+                           env=dict(os.environ, OSB_MATCH_SIMT=simt))
+        assert p.returncode == 0, p.stderr[-2000:]
+        res = json.loads([l for l in p.stdout.splitlines() if l.startswith('RESULT ')][-1][len('RESULT '):])
+        assert len(res) == 15
+        for key, (rc, err) in res.items():
+            assert rc != 0 and 'K_text' in err and 'outside 1..480' in err, (simt, key, rc, err)

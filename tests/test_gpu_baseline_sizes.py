@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from openscene_b200 import synth
+from tests import match_ref as M
 from tests.util import rel_row_err
 
 pytestmark = pytest.mark.gpu
@@ -128,10 +129,8 @@ def test_ensemble_matching_at_matterport_shape():
     s, l, fe, m = matching.match_ensemble(f3.to(DEV), f2.to(DEV), inv.to(DEV), text.to(DEV), return_features=True)
     torch.set_num_threads(16)
     sr, lr, fer, mr = om.match_ensemble(f3, f2, inv, text)
-    agree = (m.cpu() == mr)
-    assert agree.float().mean() > 0.99                                    # ties between fp16 maxima may flip
-    rows = agree.nonzero()[:, 0]
-    assert torch.equal(fe.cpu()[rows], fer[rows])
-    assert (s.float().cpu()[rows] - sr.float()[rows]).abs().max() < 1e-3 * sr.float().abs().max() + 1e-3
-    assert (l.cpu()[rows] == lr[rows]).float().mean() > 0.995
-    assert torch.equal(l.cpu(), s.float().cpu().max(1)[1])
+    # against fp64: a choice may differ only where the two maxima's bound intervals overlap (ties between fp16 maxima), the
+    # feature is the chosen row bit for bit, every score within its bound, labels by the rule; the oracle obeys the same
+    w, n_dis, gap = M.check_ensemble(s, l, fe, m, f3.to(DEV), f2.to(DEV), inv.to(DEV), text.to(DEV), 'tc')
+    print('ensemble at Matterport shape: worst', w, 'of the bound;', n_dis, 'choices differ from fp64, largest gap', gap)
+    M.check_ensemble(sr.to(DEV), lr.to(DEV), fer.to(DEV), mr.to(DEV), f3.to(DEV), f2.to(DEV), inv.to(DEV), text.to(DEV), 'tc')
