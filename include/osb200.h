@@ -122,11 +122,13 @@ int osb_kernel_map_transpose(const int32_t *nbr, int64_t n_out, int32_t K, int32
  * Generic fp32 path (CUDA cores; any channel counts).  out[o,:] = sum_k in[nbr[k][o],:] @ W[k]
  *   in   fp32 [n_in, cin] (row stride ld_in floats)     w  fp32 [K, cin, cout]
  *   out  fp32 [n_out, cout]
- *   transpose_w != 0: use W[k]^T, i.e. w is [K, cout, cin] (dgrad). */
+ *   transpose_w != 0: use W[k]^T, i.e. w is [K, cout, cin] (dgrad).
+ *   nbr NULL: the identity map (K == 1).  Refused before any launch: ld_in < cin, NULL in / w / out. */
 int osb_conv_fwd_f32(const float *in, int64_t ld_in, const int32_t *nbr, int64_t n_out, int32_t K,
                      const float *w, int32_t cin, int32_t cout, int32_t transpose_w, float *out, void *stream);
 
-/* Weight gradient: gw[k] = sum_o in[nbr[k][o],:]^T gout[o,:]   (gw fp32 [K,cin,cout], overwritten). */
+/* Weight gradient: gw[k] = sum_o in[nbr[k][o],:]^T gout[o,:]   (gw fp32 [K,cin,cout], overwritten; in rows of cin floats).
+ * nbr NULL: the identity map (K == 1).  Refused before any launch or memset: NULL in / gout / gw. */
 int osb_conv_wgrad_f32(const float *in, const int32_t *nbr, int64_t n_out, int32_t K, const float *gout,
                        int32_t cin, int32_t cout, float *gw, void *stream);
 

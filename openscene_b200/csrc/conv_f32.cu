@@ -292,6 +292,8 @@ int osb_conv_fwd_f32(const float *in, int64_t ld_in, const int32_t *nbr, int64_t
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(n_out > 0 && K >= 1 && cin >= 1 && cout >= 1, "osb_conv_fwd_f32: bad shape");
   OSB_CHECK(nbr != nullptr || K == 1, "osb_conv_fwd_f32: identity map requires K == 1");
+  OSB_CHECK(ld_in >= cin, "osb_conv_fwd_f32: ld_in %lld < cin %d", (long long)ld_in, cin);
+  OSB_CHECK(in && w && out, "osb_conv_fwd_f32: NULL buffer (in %p, w %p, out %p)", (const void *)in, (const void *)w, (void *)out);
   if (nbr != nullptr && !transpose_w && cout == THIN_COUT && cin >= 1 && cin <= 4 && ld_in == cin && K * cin * THIN_COUT * 4 <= 96 * 1024) {
     switch (cin) {                                     // the 5x5x5 stem in training mode
       case 1: return launch_fwd_thin<1>(in, nbr, n_out, K, w, out, stream);
@@ -310,6 +312,8 @@ int osb_conv_wgrad_f32(const float *in, const int32_t *nbr, int64_t n_out, int32
                        int32_t cout, float *gw, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   OSB_CHECK(n_out > 0 && K >= 1 && K <= 65535 && cin >= 1 && cout >= 1, "osb_conv_wgrad_f32: bad shape");
+  OSB_CHECK(nbr != nullptr || K == 1, "osb_conv_wgrad_f32: identity map requires K == 1");
+  OSB_CHECK(in && gout && gw, "osb_conv_wgrad_f32: NULL buffer (in %p, gout %p, gw %p)", (const void *)in, (const void *)gout, (void *)gw);
   OSB_CUDA(cudaMemsetAsync(gw, 0, sizeof(float) * (size_t)K * cin * cout, stream));
   if (nbr != nullptr && cout == THIN_COUT && cin <= 4 && K <= THIN_WG_WARPS * THIN_WG_KPW) {
     switch (cin) {

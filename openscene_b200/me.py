@@ -198,11 +198,19 @@ class SparseTensor:
         return f"SparseTensor(N={self.shape[0]}, C={self.shape[1]}, tensor_stride={self.tensor_stride})"
 
 
+def _require_f32(t, what):
+    """The CUDA-core entry points read fp32 rows: any other dtype would be reinterpreted (fp64) or read and written out of
+    bounds (fp16), so it is refused before anything launches."""
+    if t.dtype != torch.float32:
+        raise TypeError(f"openscene_b200: {what} must be float32, got {t.dtype}")
+
+
 class _RowGather(torch.autograd.Function):
     """out[r] = x[idx[r]] with idx a permutation (its inverse ``inv`` drives the backward)."""
 
     @staticmethod
     def forward(ctx, x, idx, inv):
+        _require_f32(x, 'row gather input')
         ctx.save_for_backward(idx, inv)
         x = x.contiguous()
         out = torch.empty_like(x)
@@ -241,6 +249,8 @@ def cat(*tensors):
 # ------------------------------------------------------------------------------------------------
 def _conv_raw(x, kmap, w3, n_out, transpose_w=False):
     """x fp32 [n_in, cin]; w3 fp32 [K, cin, cout] ([K, cout, cin] when transpose_w)."""
+    _require_f32(x, 'convolution input')
+    _require_f32(w3, 'convolution kernel')
     x = x.contiguous()
     w3 = w3.contiguous()
     K = w3.shape[0]
@@ -311,6 +321,9 @@ class SparseConvFunction(torch.autograd.Function):
                 kt = kmap.transposed() if kmap is not None else None
                 gx = _conv_raw(gout, kt, w3, ctx.n_in, transpose_w=True)
             if ctx.needs_input_grad[1]:
+                _require_f32(x, 'convolution input')
+                _require_f32(gout, 'convolution output gradient')
+                _require_f32(w3, 'convolution kernel')
                 gw = torch.empty_like(w3)
                 nbr = kmap.nbr if kmap is not None else None
                 C.call('osb_conv_wgrad_f32', C.ptr(x.contiguous()), C.ptr(nbr), gout.shape[0], K, C.ptr(gout),

@@ -1,6 +1,8 @@
-"""fp64 references and error bounds for the tensor-core convolution entry points of libosb200, shared by
+"""fp64 references and error bounds for the convolution entry points of libosb200, shared by
 tests/test_gpu_launch_replay.py (every launch of the engine replayed on its own operands), tests/test_gpu_conv_exact.py
-(bit-exact probes) and their CPU self-check tests/test_replay_ref_cpu.py.  Every function runs on CPU or CUDA tensors.
+(bit-exact probes of the tensor-core arithmetic), tests/test_gpu_conv_f32.py and tests/test_gpu_me_module_exact.py (the
+CUDA-core kernels and the module surface) and their CPU self-checks tests/test_replay_ref_cpu.py and
+tests/test_f32conv_ref_cpu.py.  Every function runs on CPU or CUDA tensors.
 
 Bounds (DESIGN.md section 2): a tensor-core result y and its fp64 reference y^ computed from the operands the launch read
 satisfy, element by element,
@@ -49,6 +51,79 @@ def c_wgrad(n_out, K, cin, cout):
 def c_fma(n_terms):
     """fp32 FMA chains on CUDA cores (stem, osb_conv_fwd_f32): fp32 operands, one rounding of 2^-24 per term and epilogue"""
     return 2.0 ** 16 * (n_terms + 3) * 2.0 ** -24
+
+
+# ------------------------------------------------------------------ CUDA-core fp32 kernels (csrc/conv_f32.cu)
+# Every output element of the CUDA-core kernels is an fp32 FMA chain, possibly followed by float atomic adds of per-block
+# partials in any order.  To first order each rounding costs 2^-24 of the magnitudes it has summed, so with `depth` the
+# longest chain of roundings any one term passes through, |y - y^| <= (depth + 3) 2^-24 A (c_fma(depth) in units of
+# 2^-16 A), valid while depth 2^-24 << 1.
+THIN_COUT, THIN_SMEM_MAX = 32, 96 * 1024              # k_conv_fwd_thin: lane = output channel, weights in shared memory
+WG_ROWS = 4096                                         # k_conv_wgrad_f32: rows per block (one atomic partial each)
+THIN_WG_ROWS, THIN_WG_GRID, THIN_WG_KMAX = 128, 132 * 4, 8 * 16    # k_conv_wgrad_thin: chunk rows, grid cap, offsets
+
+
+def f32_dispatch(entry, cin, cout, K, has_nbr, ld_in=None, transpose_w=False):
+    """which kernel osb_conv_fwd_f32 ('fwd') / osb_conv_wgrad_f32 ('wgrad') launches for these arguments:
+    'fwd_thin', 'fwd_generic', 'wgrad_thin' or 'wgrad_generic' (a restatement of the host code's dispatch)"""
+    if entry == 'fwd':
+        ld_in = cin if ld_in is None else ld_in
+        thin = (has_nbr and not transpose_w and cout == THIN_COUT and 1 <= cin <= 4 and ld_in == cin
+                and K * cin * THIN_COUT * 4 <= THIN_SMEM_MAX)
+        return 'fwd_thin' if thin else 'fwd_generic'
+    assert entry == 'wgrad'
+    thin = has_nbr and cout == THIN_COUT and cin <= 4 and K <= THIN_WG_KMAX
+    return 'wgrad_thin' if thin else 'wgrad_generic'
+
+
+def f32_fwd_depth(K, cin):
+    """both forwards: one thread owns an output element and runs K cin FMAs in one chain (absent neighbours and padded
+    channels add exact zeros)"""
+    return K * cin
+
+
+def thin_wgrad_grid(n_out):
+    return min(-(-n_out // THIN_WG_ROWS), THIN_WG_GRID)
+
+
+def f32_wgrad_depth(kernel, n_out):
+    """generic: at most WG_ROWS FMAs in a block's row chunk, then ceil(n_out / WG_ROWS) atomic adds in any order;
+    thin: a block walks ceil(n_chunks / grid) chunks of THIN_WG_ROWS rows in one register, then one atomic add per block"""
+    if kernel == 'wgrad_generic':
+        return min(n_out, WG_ROWS) + -(-n_out // WG_ROWS)
+    assert kernel == 'wgrad_thin'
+    n_chunks = -(-n_out // THIN_WG_ROWS)
+    grid = thin_wgrad_grid(n_out)
+    return -(-n_chunks // grid) * THIN_WG_ROWS + grid
+
+
+def f32_depth(kernel, K, cin, n_out):
+    return f32_fwd_depth(K, cin) if kernel.startswith('fwd') else f32_wgrad_depth(kernel, n_out)
+
+
+# dyadic probe operands: features {0, +-1, +-2} 2^-3, weights and gradients {0, +-1, +-2, +-3} 2^-4, so every product is a
+# multiple of 2^-7 and an fp32 accumulation is exact in any order while sum |terms| < 2^24 x 2^-7
+PROBE_X, PROBE_W, PROBE_GRID = (0., 1., -1., 2., -2.), (0., 1., -1., 2., -2., 3., -3.), 2.0 ** -7
+
+
+def probe_values(shape, vals, scale, generator=None, device='cpu'):
+    v = torch.tensor(vals, dtype=torch.float32, device=device) * scale
+    return v[torch.randint(len(vals), shape, generator=generator, device=device)]
+
+
+def probe_x(shape, generator=None, device='cpu'):
+    return probe_values(shape, PROBE_X, 2.0 ** -3, generator, device)
+
+
+def probe_w(shape, generator=None, device='cpu'):
+    return probe_values(shape, PROBE_W, 2.0 ** -4, generator, device)
+
+
+def binade_rows(n, c, spread=8, generator=None, device='cpu'):
+    """random fp32 rows whose magnitudes span 2 spread + 1 binades (one power-of-two scale per row)"""
+    x = torch.randn((n, c), generator=generator, device=device)
+    e = torch.randint(-spread, spread + 1, (n, 1), generator=generator, device=device).float()
+    return x * torch.exp2(e)
 
 
 # ------------------------------------------------------------------ split rows

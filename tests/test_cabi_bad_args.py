@@ -87,3 +87,36 @@ def test_match_entry_points_refuse_text_counts_outside_1_to_480_on_both_routes()
         assert len(res) == 15
         for key, (rc, err) in res.items():
             assert rc != 0 and 'K_text' in err and 'outside 1..480' in err, (simt, key, rc, err)
+
+
+_CONV_CHILD = r'''
+import json, sys
+sys.path.insert(0, sys.argv[1])
+from openscene_b200 import _cabi as C
+L = C.lib()
+out = {}
+def run(name, *args):
+    return [getattr(L, name)(*args), (L.osb_last_error() or b'').decode()]
+# valid shapes (n_out 10, cin 3, cout 32, K 1 over the identity map); only the named argument is wrong.  NULL buffers
+# throughout, so nothing could be launched even if a refusal were missing.
+out['fwd:ld_in<cin'] = run('osb_conv_fwd_f32', None, 2, None, 10, 1, None, 3, 32, 0, None, None)
+out['fwd:NULL buffers'] = run('osb_conv_fwd_f32', None, 3, None, 10, 1, None, 3, 32, 0, None, None)
+out['fwd:identity map, K 27'] = run('osb_conv_fwd_f32', None, 3, None, 10, 27, None, 3, 32, 0, None, None)
+out['wgrad:identity map, K 27'] = run('osb_conv_wgrad_f32', None, None, 10, 27, None, 3, 32, None, None)
+out['wgrad:NULL buffers'] = run('osb_conv_wgrad_f32', None, None, 10, 1, None, 3, 32, None, None)
+print('RESULT ' + json.dumps(out))
+'''
+
+
+def test_fp32_convolutions_refuse_bad_buffers_and_maps_with_valid_shapes():
+    """osb_conv_fwd_f32 / osb_conv_wgrad_f32 refuse, on the host and before the weight gradient's memset, a row stride
+    below cin, NULL operand buffers and an identity map with K != 1; each message names its cause"""
+    p = subprocess.run([sys.executable, '-c', _CONV_CHILD, ROOT], capture_output=True, text=True, timeout=300)
+    assert p.returncode == 0, p.stderr[-2000:]
+    res = json.loads([l for l in p.stdout.splitlines() if l.startswith('RESULT ')][-1][len('RESULT '):])
+    want = {'fwd:ld_in<cin': 'ld_in 2 < cin 3', 'fwd:NULL buffers': 'NULL buffer',
+            'fwd:identity map, K 27': 'identity map requires K == 1', 'wgrad:identity map, K 27': 'identity map requires K == 1',
+            'wgrad:NULL buffers': 'NULL buffer'}
+    assert set(res) == set(want)
+    for key, (rc, err) in res.items():
+        assert rc != 0 and want[key] in err, (key, rc, err)
