@@ -105,7 +105,8 @@ __global__ void __launch_bounds__(BN_THREADS) k_bn_finalize(const uint8_t *__res
       const double pivot = (double)join_bf16(*reinterpret_cast<const __nv_bfloat16 *>(row0),
                                              *reinterpret_cast<const __nv_bfloat16 *>(row0 + 64));
       const double dm = t1 / (double)n;
-      const double var = fmax(t2 / (double)n - dm * dm, 0.0);        // biased: what normalises the batch
+      const double v = t2 / (double)n - dm * dm;
+      const double var = v < 0.0 ? 0.0 : v;                          // biased: what normalises the batch; NaN stays NaN
       const double mean = pivot + dm;
       const double istd = 1.0 / sqrt(var + eps);
       const double sc = (double)weight[cc] * istd;
@@ -118,6 +119,13 @@ __global__ void __launch_bounds__(BN_THREADS) k_bn_finalize(const uint8_t *__res
     __syncthreads();
   }
   if (threadIdx.x == 0) *num_batches_tracked = tracked;
+}
+
+// torch.relu: NaN passes through (fmaxf would turn it into 0); otherwise the same instruction as fmaxf(y, 0)
+__device__ inline float relu_nan(float y) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(y), "f"(0.f));
+  return r;
 }
 
 // grid (row chunks, C/32): RES 0 = no residual, 1 = split rows, 2 = split rows normalised by res_scale / res_shift
@@ -145,7 +153,7 @@ __global__ void __launch_bounds__(BN_THREADS) k_bn_apply(const uint8_t *x, uint8
       float y = fmaf(v[j], sc[j], sh[j]);
       if (RES == 1) y += rv[j];
       if (RES == 2) y += fmaf(rv[j], rsc[j], rsh[j]);
-      v[j] = RELU ? fmaxf(y, 0.f) : y;
+      v[j] = RELU ? relu_nan(y) : y;
     }
     store4(y_out + off, q, v);
   }
@@ -158,7 +166,8 @@ static void launch_apply(dim3 grid, cudaStream_t st, const void *x, void *y, int
                                                      res_scale, res_shift);
 }
 
-// ---- backward of y = act(BN(z) + r), BN with batch statistics: g' = g [y > 0] (or g without ReLU), x^ = (z - mean) invstd,
+// ---- backward of y = act(BN(z) + r), BN with batch statistics: g' = g [not y <= 0] (torch's threshold_backward: a NaN output
+//      passes its gradient; g without ReLU), x^ = (z - mean) invstd,
 //      dbias = sum g', dweight = sum g' x^, dz = weight invstd (g' - sum g' / n - x^ sum g' x^ / n)
 
 // grid (row blocks, C/32).  part: [row block][2][C] fp64 = (sum of g', sum of g' x^)
@@ -185,7 +194,7 @@ __global__ void __launch_bounds__(BN_THREADS) k_bn_bwd_partial(const uint8_t *__
     if (MASK) load4(y + off, q, yv);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const double gp = (MASK && !(yv[j] > 0.f)) ? 0.0 : (double)gv[j];
+      const double gp = (MASK && yv[j] <= 0.f) ? 0.0 : (double)gv[j];
       a1[j] += gp;
       a2[j] = fma(gp, ((double)zv[j] - mu[j]) * is[j], a2[j]);
     }
@@ -259,7 +268,7 @@ __global__ void __launch_bounds__(BN_THREADS) k_bn_bwd_apply(const uint8_t *__re
     if (GP == 2) load4(gp_out + off, q, pv);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const float gp = (MASK && !(yv[j] > 0.f)) ? 0.f : gv[j];
+      const float gp = (MASK && yv[j] <= 0.f) ? 0.f : gv[j];
       const float xh = (zv[j] - mu[j]) * is[j];
       if (GP == 1) pv[j] = gp;
       if (GP == 2) pv[j] += gp;

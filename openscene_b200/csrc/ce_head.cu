@@ -2,7 +2,7 @@
 // followed by CrossEntropyLoss(ignore_index) with the mean over labelled rows and the argmax the training mIoU needs
 // (run/train_mink.py's step).  The logits never go to memory.
 //
-//   osb_ce_head_fwd  per row: z = x W (fp32), lse = log sum exp z, pred = first argmax, nll = lse - z[label];
+//   osb_ce_head_fwd  per row: z = x W (fp32), lse = log sum exp z, pred = first argmax (first NaN), nll = lse - z[label];
 //                    loss = sum of nll over labelled rows / n_valid (fp64 sum, per-block partials merged in a fixed order).
 //   osb_ce_head_bwd  d = (softmax(z) - onehot(label)) g / n_valid on labelled rows (0 elsewhere), dx = d W^T (split rows),
 //                    dW = sum_r x_r^T d_r (fp32 per-split partials, merged in fp64 in a fixed order).
@@ -142,7 +142,8 @@ __global__ void __launch_bounds__(CE_THREADS) k_ce_fwd(const uint8_t *__restrict
         const int cc = 32 * j + q;
         if (cc < c) {
           mc = fmaxf(mc, z[q]);
-          if (z[q] > best) { best = z[q]; arg = cc; }          // strict: the first maximum
+          // strict: the first maximum; a NaN beats everything and is never beaten (torch's max(1)[1]: the first NaN)
+          if (z[q] > best || (z[q] != z[q] && best == best)) { best = z[q]; arg = cc; }
           if (cc == lab) { zl = z[q]; found = true; }
         }
       }

@@ -7,6 +7,7 @@ import torch
 import torch.nn.functional as F
 
 from openscene_b200 import _cabi as C
+from tests import norm_ref as NR
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -91,8 +92,12 @@ def test_bn_backward_kernels_match_fp64_autograd(n, c, form, relu):
     dw_ref, db_ref = (gp_ref * xh).sum(0), gp_ref.sum(0)
     same = ((y > 0) == (yy.detach() > 0)).all(1) if relu else torch.ones(n, dtype=torch.bool, device=DEV)
     assert float(dw[0]) != 0.0 and float(_joined(dz_rows, c)[:, 0].abs().max()) == 0.0   # weight 0: dz 0
-    assert float((dw.double() - dw_ref).abs().max()) <= 1e-4 * float(dw_ref.abs().max())
-    assert float((db.double() - db_ref).abs().max()) <= 1e-4 * float(db_ref.abs().max())
+    # dweight / dbias per channel against the operands the launch read (the kernel's mask, saved mean / invstd):
+    # tests/norm_ref.py's depth term plus one fp32 rounding
+    bw = NR.bn_backward(y if relu else None, gin, z, mu, istd, w)
+    rb0 = NR.reduce_bounds(bw)
+    assert bool(((dw.double() - bw['t2']).abs() <= rb0['dweight']).all())
+    assert bool(((db.double() - bw['t1']).abs() <= rb0['dbias']).all())
     dz_ref = ww.detach() * torch.rsqrt(var + 1e-5) * (gp_ref - db_ref / n - xh * dw_ref / n)
     dz = _joined(dz_rows, c).double()
     a = (ww.detach() * torch.rsqrt(var + 1e-5)).abs()
@@ -111,7 +116,11 @@ def test_bn_backward_kernels_match_fp64_autograd(n, c, form, relu):
     assert all(torch.equal(p, q) for p, q in zip(first, second))
     C.call('osb_bn_backward_reduce', y_arg, g_rows.data_ptr(), z_rows.data_ptr(), n, c, mu.data_ptr(), istd.data_ptr(),
            sums.data_ptr(), dw.data_ptr(), db.data_ptr(), 1, ws.data_ptr(), ws_bytes, C.stream_ptr())
-    assert torch.allclose(dw, 2 * first[0], rtol=1e-6, atol=0) and torch.allclose(db, 2 * first[1], rtol=1e-6, atol=0)
+    # accumulate: one fp32 rounding of prev + t (tests/norm_ref.py).  prev = fp32(t) here, so a double rounding
+    # prev + fp32(t) = fp32(2 t) would not show; tests/test_gpu_bn_exact.py accumulates onto independent values
+    rb = NR.reduce_bounds(bw, first[0], first[1])
+    assert bool(((dw.double() - rb['dw_ref']).abs() <= rb['dweight']).all())
+    assert bool(((db.double() - rb['db_ref']).abs() <= rb['dbias']).all())
     C.call('osb_bn_backward_apply', y_arg, g_rows.data_ptr(), z_rows.data_ptr(), n, c, mu.data_ptr(),
            istd.data_ptr(), w.data_ptr(), sums.data_ptr(), dz_rows.data_ptr(), gp_rows.data_ptr(), 1, C.stream_ptr())
     gp2 = _joined(gp_rows, c).double()

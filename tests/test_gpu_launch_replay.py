@@ -39,10 +39,10 @@ dev = torch.device('cuda:0')
 
 # entry points passed through unreplayed, each owned by another test
 PASS = {
-    'osb_bn_batch_stats', 'osb_bn_apply_split', 'osb_bn_batch_stats_save', 'osb_bn_apply_split_out',   # test_gpu_bn_batch_stats.py
-    'osb_bn_backward_reduce',                                                                           # test_gpu_bn_backward.py
+    'osb_bn_batch_stats', 'osb_bn_apply_split', 'osb_bn_batch_stats_save', 'osb_bn_apply_split_out',   # test_gpu_norm_replay.py
+    'osb_bn_backward_reduce',                                                                           # test_gpu_norm_replay.py
     'osb_bn_stats_workspace_bytes',
-    'osb_ce_head_fwd', 'osb_ce_head_bwd', 'osb_ce_head_workspace_bytes',                                # test_gpu_ce_head.py
+    'osb_ce_head_fwd', 'osb_ce_head_bwd', 'osb_ce_head_workspace_bytes',                                # test_gpu_norm_replay.py
     'osb_f32_to_split', 'osb_split_to_f32', 'osb_gather_rows_f32',              # test_gpu_conv_tc.py, test_gpu_engine.py
     'osb_kernel_map_build', 'osb_kernel_map_build_grid', 'osb_kernel_map_transpose', 'osb_hash_build',  # test_gpu_coords.py
     'osb_coordset_build', 'osb_coordset_stride', 'osb_coordset_pyramid', 'osb_coordset_workspace_bytes',
