@@ -435,6 +435,44 @@ int osb_feature_remap(const uint8_t *mask_full, int64_t n_pts, const int64_t *vo
                       int64_t m_rows, int32_t row_bytes, int32_t keep_all, uint8_t *mask_vox, void *feat_out,
                       int64_t *n_out_host, void *ws, size_t ws_bytes, void *stream);
 
+/* ------------------------------------------------------------- training augmentation (dataset/augmentation.py)
+ * The random draws stay on the host in the reference's order; these calls do the per-point / per-voxel arithmetic with
+ * NumPy's rounding, bit for bit.  dtype codes: 0 fp32, 1 fp64, 2 int32.  None of them synchronises.
+ *   osb_aug_minmax        minmax out fp64 [2c] DEVICE = column minima then maxima of x [n,c] (rows != NULL: of
+ *                         x[rows[i]]), NaN-propagating like np.min / np.max; 1 <= c <= 4;
+ *                         ws osb_aug_minmax_workspace_bytes(c) bytes
+ *   osb_aug_blur          in place on grid fp32 [X,Y,Z,ch]: ElasticDistortion's smoothing = scipy.ndimage.convolve with
+ *                         the float32(1/3) 3-tap box along x, y, z, twice, mode='constant' (double accumulation over
+ *                         taps -1, 0, +1 from 0.0, one rounding to fp32 per pass); tmp is scratch of the same size
+ *   osb_aug_elastic_interp out fp64 [n,3] = p + RegularGridInterpolator(axes, noise, bounds_error=0, fill_value=0)(p)
+ *                         * magnitude for pts fp32 / fp64 [n,3], noise fp32 [X,Y,Z,3], axes fp64 [X+Y+Z] DEVICE
+ *   osb_aug_input_transforms  one pass over n voxels (feats / labels read at rows[v] when rows != NULL):
+ *                         stages OSB_AUG_*; params_host fp64 [8] = (1 - blend, blend, tr[3], jitter_std * 255, hue,
+ *                         saturation ratio); coords_max fp64 [3] DEVICE (for the flips), feats_minmax fp64 [6] DEVICE
+ *                         (auto-contrast), jitter fp64 [n,3] DEVICE raw standard normals.  Outputs, any may be NULL:
+ *                         coords_out / feats_out [n,3] in the input types; item_coords int32 [n,4] = (batch_index,
+ *                         x, y, z); item_feats fp32 [n,3] (float(f) / 127.5 - 1 with OSB_AUG_INPUT_COLOR, else 1);
+ *                         item_labels int64 [n]. */
+#define OSB_AUG_FLIP_X 1
+#define OSB_AUG_FLIP_Y 2
+#define OSB_AUG_AUTOCONTRAST 4
+#define OSB_AUG_TRANSLATE 8
+#define OSB_AUG_JITTER 16
+#define OSB_AUG_HUE_SAT 32
+#define OSB_AUG_INPUT_COLOR 64
+#define OSB_AUG_ALL 127
+size_t osb_aug_minmax_workspace_bytes(int32_t c);
+int osb_aug_minmax(const void *x, int32_t dtype, const int64_t *rows, int64_t n, int32_t c, double *minmax, void *ws,
+                   size_t ws_bytes, void *stream);
+int osb_aug_blur(float *grid, float *tmp, int32_t X, int32_t Y, int32_t Z, int32_t ch, void *stream);
+int osb_aug_elastic_interp(const void *pts, int32_t pts_is_f64, int64_t n, const float *noise, int32_t X, int32_t Y,
+                           int32_t Z, const double *axes, double magnitude, double *out, void *stream);
+int osb_aug_input_transforms(const void *coords, int32_t coords_dtype, const void *feats, int32_t feats_is_f64,
+                             const uint8_t *labels, const int64_t *rows, int64_t n, const double *coords_max,
+                             const double *feats_minmax, const double *jitter, const double *params_host, int32_t stages,
+                             int32_t batch_index, void *coords_out, void *feats_out, int32_t *item_coords,
+                             float *item_feats, int64_t *item_labels, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -78,6 +78,12 @@ SIGNATURES = {
     'osb_feature_remap': (c_int, [P, I64, P, I64, P, I64, I32, I32, P, P, POINTER(I64), P, SZ, P]),
     'osb_confusion_accumulate': (c_int, [P, P, I32, I64, I32, I32, I32, P, P, P]),
     'osb_intersection_union': (c_int, [P, P, I32, I64, I32, I32, P, P]),
+    'osb_aug_minmax_workspace_bytes': (SZ, [I32]),
+    'osb_aug_minmax': (c_int, [P, I32, P, I64, I32, P, P, SZ, P]),
+    'osb_aug_blur': (c_int, [P, P, I32, I32, I32, I32, P]),
+    'osb_aug_elastic_interp': (c_int, [P, I32, I64, P, I32, I32, I32, P, c_double, P, P]),
+    'osb_aug_input_transforms': (c_int, [P, I32, P, I32, P, P, I64, P, P, P, POINTER(c_double), I32, I32, P, P, P, P, P,
+                                         P]),
 }
 
 

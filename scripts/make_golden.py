@@ -17,7 +17,11 @@
    synthetic scene / fused-feature files written to a scratch directory (``SharedArray`` stubbed; ``torch.load`` given
    the ``weights_only=False`` default of the PyTorch the reference targets), plus the 4x4 matrix its voxeliser drew.
 
-Usage: python scripts/make_golden.py [voxelizer] [unet] [fusion] [metric] [loader]
+6. augment_*.npz   : the reference's own ``dataset/augmentation.py`` transforms and the ``aug=True`` items of its
+   ``Point3DLoader`` / ``FusedFeatureLoader`` (same stubs as 5.) for seeded inputs.  Each case stores its inputs, the
+   seed of both global generators, the outputs and the next draws of ``random`` and ``np.random`` after the call.
+
+Usage: python scripts/make_golden.py [voxelizer] [unet] [fusion] [metric] [loader] [augment]
 """
 import collections
 import collections.abc
@@ -223,8 +227,158 @@ def golden_loader():
         shutil.rmtree(tmp, ignore_errors=True)
 
 
+def _seed_where(pred, start=0):
+    """first seed >= start whose Python `random` stream satisfies pred(random.Random(seed))"""
+    import random
+    s = start
+    while not pred(random.Random(s)):
+        s += 1
+    return s
+
+
+def _after_draws():
+    import random
+    return np.array([random.random() for _ in range(3)]), np.random.rand(3)
+
+
+def golden_augment():
+    """augment_{elastic,colour,point,fused}.npz: case k is stored under keys 'c<k>_*'."""
+    import functools
+    import random
+    import shutil
+    import tempfile
+    collections.Sequence = collections.abc.Sequence
+    collections.Iterable = collections.abc.Iterable
+    _stub_modules('SharedArray')
+    sys.path.insert(0, REF)
+    import dataset.augmentation as t
+    from dataset.feature_loader import FusedFeatureLoader
+    from dataset.point_loader import Point3DLoader
+    from openscene_b200 import synth
+
+    def run(store, k, seed, fn, **inputs):
+        random.seed(seed)
+        np.random.seed(seed)
+        out = fn(**{a: (b.copy() if isinstance(b, np.ndarray) else b) for a, b in inputs.items()})
+        nxt_py, nxt_np = _after_draws()
+        store[f'c{k}_seed'] = np.int64(seed)
+        for a, b in inputs.items():
+            store[f'c{k}_in_{a}'] = np.asarray(b)
+        for a, b in out.items():
+            store[f'c{k}_out_{a}'] = np.asarray(b)
+        store[f'c{k}_next_py'], store[f'c{k}_next_np'] = nxt_py, nxt_np
+
+    fires = lambda r: r.random() < 0.95            # noqa: E731
+    skips = lambda r: r.random() >= 0.95           # noqa: E731
+
+    # ---- elastic: float32 / float64 rooms, 1 and 2 points, the gate both ways, points on grid nodes and edges
+    el = {}
+    ed = t.ElasticDistortion(((0.2, 0.4), (0.8, 1.6)))
+    room = synth.room_points((2.0, 1.6, 1.0), 3, 0.04, seed=5)
+    room = room[::max(1, len(room) // 3000)]
+    clouds = [room.astype(np.float32), room, np.array([[0.3, -1.2, 2.5]]), np.array([[0.0, 0.0, 0.0], [0.4, 0.6, 0.2]],
+              dtype=np.float32), np.array([[0.0, 0.0, 0.0], [1.0, 0.6, 0.4], [0.2, 0.4, 0.6], [0.6, 0.2, 0.8]])]
+    k = 0
+    for ci, cl in enumerate(clouds):
+        seed = _seed_where(fires, 100 * ci)
+        run(el, k, seed, lambda pointcloud: {'coords': ed(pointcloud)}, pointcloud=cl)
+        k += 1
+    run(el, k, _seed_where(skips), lambda pointcloud: {'coords': ed(pointcloud)}, pointcloud=clouds[0])
+    k += 1
+    run(el, k, 7, lambda pointcloud: {'coords': t.ElasticDistortion(None)(pointcloud)}, pointcloud=clouds[1])
+    np.savez_compressed(os.path.join(OUT, 'augment_elastic.npz'), n=np.int64(k + 1), **el)
+    print('augment elastic cases', k + 1)
+
+    # ---- colour / flip transforms one at a time: float32 and float64, both gate outcomes, clip edges, every hue sextant
+    rng = np.random.RandomState(61)
+    edge = np.array([[0, 0, 0], [255, 255, 255], [255, 0, 0], [255, 255, 0], [0, 255, 0], [0, 255, 255], [0, 0, 255],
+                     [255, 0, 255], [128, 128, 128], [254.9, 0.1, 3.0], [255, 0, 1], [1, 0, 255], [7.5, 7.5, 7.5],
+                     [200, 10, 10], [10, 200, 10], [10, 10, 200]], dtype=np.float64)
+    cols64 = np.concatenate([edge, rng.rand(400, 3) * 255])
+    coords = np.floor(rng.rand(len(cols64), 3) * [40, 30, 12])
+    const = np.full((50, 3), 127.5)
+    tf = {'flip': (t.RandomHorizontalFlip('z', False), 0.95), 'autocontrast': (t.ChromaticAutoContrast(), 0.2),
+          'translation': (t.ChromaticTranslation(0.1), 0.95), 'jitter': (t.ChromaticJitter(0.05), 0.95),
+          'hue_sat': (t.HueSaturationTranslation(0.5, 0.2), None)}
+    co, k = {}, 0
+    kinds = []
+    for name, (tr, p) in tf.items():
+        outcomes = [True] if p is None else [True, False]
+        for dt in (np.float32, np.float64):
+            for on in outcomes:
+                for extra in range(2 if name in ('flip', 'hue_sat') else 1):
+                    gate = (lambda r, p=p: r.random() < p) if on else (lambda r, p=p: r.random() >= p)
+                    seed = _seed_where(gate if p is not None else (lambda r: True), 1000 * k + 17 * extra)
+                    fn = lambda coords, feats, labels, tr=tr: dict(zip(('coords', 'feats', 'labels'), tr(coords, feats, labels)))
+                    run(co, k, seed, fn, coords=coords.astype(dt), feats=cols64.astype(dt), labels=np.arange(len(cols64)) % 20)
+                    kinds.append(name)
+                    k += 1
+    for dt in (np.float32, np.float64):                    # the constant-colour scene through the whole chain
+        chain = t.Compose([t.RandomHorizontalFlip('z', False), t.ChromaticAutoContrast(), t.ChromaticTranslation(0.1),
+                           t.ChromaticJitter(0.05), t.HueSaturationTranslation(0.5, 0.2)])
+        seed = _seed_where(lambda r: r.random() < 0.95 and [r.random() for _ in range(2)] and r.random() < 0.2)
+        fn = lambda coords, feats, labels, chain=chain: dict(zip(('coords', 'feats', 'labels'), chain(coords, feats, labels)))
+        with np.errstate(invalid='ignore', divide='ignore'):
+            run(co, k, seed, fn, coords=coords[:50].astype(dt), feats=const.astype(dt), labels=np.arange(50) % 20)
+        kinds.append('chain')
+        k += 1
+    np.savez_compressed(os.path.join(OUT, 'augment_colour.npz'), n=np.int64(k), kinds=np.array(kinds), **co)
+    print('augment colour cases', k)
+
+    # ---- loader items through the reference's own loaders
+    orig_load = torch.load
+    torch.load = functools.partial(orig_load, weights_only=False)
+    tmp = tempfile.mkdtemp(prefix='osb_golden_aug_')
+    try:
+        pt, fu = {}, {}
+        cases = [dict(n=3000, dt=np.float32, color=False, seed=71), dict(n=3000, dt=np.float64, color=True, seed=72),
+                 dict(n=2500, dt=np.float32, color=True, seed=73, const=True), dict(n=1, dt=np.float32, color=True, seed=74),
+                 dict(n=2, dt=np.float64, color=True, seed=75)]
+        for k, c in enumerate(cases):
+            rng = np.random.RandomState(c['seed'])
+            n = c['n']
+            locs = (rng.rand(n, 3) * np.array([2.4, 2.0, 1.2])).astype(c['dt'])
+            colors = (rng.rand(n, 3) * 2 - 1).astype(c['dt'])
+            if c.get('const'):
+                colors[:] = 0
+            else:
+                colors[:3] = np.array([[-1, -1, -1], [1, 1, 1], [1, -1, 0]], dtype=c['dt'])[:min(3, n)]
+            labels = rng.randint(0, 20, n).astype(np.float64)
+            labels[rng.rand(n) < 0.1] = -100
+            root = os.path.join(tmp, f'p{k}', 'scannet_3d')
+            os.makedirs(os.path.join(root, 'train'))
+            featdir = os.path.join(tmp, f'p{k}', 'feat')
+            os.makedirs(featdir)
+            torch.save((locs, colors, labels), os.path.join(root, 'train', 'scene0000_00_vh_clean_2.pth'))
+            mask_full = torch.from_numpy(rng.rand(n) < 0.5)
+            mask_full[0] = True
+            feat = torch.from_numpy(rng.randn(int(mask_full.sum()), 16).astype(np.float16))
+            torch.save({'feat': feat, 'mask_full': mask_full}, os.path.join(featdir, 'scene0000_00_0.pt'))
+            lab_in = labels.copy()
+            lab_in[lab_in == -100] = 255
+            lab_in = lab_in.astype(np.uint8)
+            pl = Point3DLoader(datapath_prefix=root, voxel_size=0.05, split='train', aug=True, input_color=c['color'])
+            fl = FusedFeatureLoader(datapath_prefix=root, datapath_prefix_feat=featdir, voxel_size=0.05, split='train',
+                                    aug=True, input_color=c['color'])
+            ins = dict(locs=locs, feats=(colors + 1.) * 127.5, labels=lab_in, colors=colors, input_color=c['color'])
+            fns = {'point': lambda **_: dict(zip(('coords', 'feats', 'labels'), pl[0])),
+                   'fused': lambda **_: dict(zip(('coords', 'feats', 'labels', 'feat_3d', 'mask'), fl[0]))}
+            for store, kind in ((pt, 'point'), (fu, 'fused')):
+                seed = _seed_where(fires, 10 * c['seed'] + (kind == 'fused'))
+                run(store, k, seed, fns[kind], **ins)
+                if kind == 'fused':
+                    store[f'c{k}_in_feat'], store[f'c{k}_in_mask_full'] = feat.numpy(), mask_full.numpy()
+            print('augment items', k, 'points', n, 'voxels', pt[f'c{k}_out_coords'].shape[0])
+        np.savez_compressed(os.path.join(OUT, 'augment_point.npz'), n=np.int64(len(cases)), **pt)
+        np.savez_compressed(os.path.join(OUT, 'augment_fused.npz'), n=np.int64(len(cases)), **fu)
+    finally:
+        torch.load = orig_load
+        shutil.rmtree(tmp, ignore_errors=True)
+
+
 if __name__ == '__main__':
     os.makedirs(OUT, exist_ok=True)
-    todo = sys.argv[1:] or ['voxelizer', 'unet', 'fusion', 'metric', 'loader']
+    todo = sys.argv[1:] or ['voxelizer', 'unet', 'fusion', 'metric', 'loader', 'augment']
     for nm in todo:
-        {'voxelizer': golden_voxelizer, 'unet': golden_unet, 'fusion': golden_fusion, 'metric': golden_metric, 'loader': golden_loader}[nm]()
+        {'voxelizer': golden_voxelizer, 'unet': golden_unet, 'fusion': golden_fusion, 'metric': golden_metric, 'loader': golden_loader,
+         'augment': golden_augment}[nm]()
