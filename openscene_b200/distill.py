@@ -93,10 +93,10 @@ def distill_step(model, optimizer, coords, feats, feat_3d, mask, loss_type='cosi
 def fused_distill_step(engine, optimizer, coords, feats, feat_3d, mask, loss_type='cosine', translate=True):
     """``distill_step`` on the fused engine: the same random translation, loss, zero_grad, backward and optimiser step, with
     the forward and backward of ``engine.forward_train(..., rows=mask)`` (a ``FusedMinkUNet(model, batch_stats=True)``).
-    Single process only: DistributedDataParallel wraps ``model.forward``, which the engine bypasses."""
-    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-        raise RuntimeError("fused_distill_step: the fused engine does not all-reduce gradients (world size > 1); "
-                           "use distill_step on the DistributedDataParallel model")
+    With more than one process, the engine must all-reduce the gradients itself: build it with
+    ``process_group=dist.group.WORLD`` (a DistributedDataParallel wrapper's forward, which the engine bypasses, never runs).
+    The loss stays per rank, as in run/distill.py."""
+    refuse_local_engine(engine, 'fused_distill_step')
     if translate:
         coords = coords.clone()
         coords[:, 1:4] += (torch.rand(3) * 100).type_as(coords)
@@ -107,6 +107,16 @@ def fused_distill_step(engine, optimizer, coords, feats, feat_3d, mask, loss_typ
     loss.backward()
     optimizer.step()
     return loss.detach()
+
+
+def refuse_local_engine(engine, what):
+    """Refuse a fused engine that keeps its gradients local when more than one process trains."""
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        pg = engine.process_group
+        if pg is None or dist.get_world_size(group=pg) < 2:
+            raise RuntimeError(f"{what}: the fused engine all-reduces gradients only when built with a process group "
+                               f"(world size {dist.get_world_size()}): FusedMinkUNet(model, batch_stats=True, "
+                               f"process_group=dist.group.WORLD)")
 
 
 def wrap_ddp(model, device=None):

@@ -20,10 +20,17 @@ under no_grad): every BatchNorm normalises with the statistics of the current ba
 ``osb_bn_apply_split`` normalises them in place, with the ReLU and the BasicBlock residual (the downsample branch's raw output
 is normalised inside that same pass).  Layers run one launch each (a full reduction separates a layer from its consumer, so
 the persistent chain has nothing to fuse) (tests/test_gpu_bn_batch_stats.py).
+
+``FusedMinkUNet(model, batch_stats=True, process_group=pg)`` trains data-parallel over ``pg`` as DistributedDataParallel does
+with its defaults: rank 0's parameters and buffers are broadcast at construction, its BatchNorm running buffers before a
+forward that follows a grad-enabled one, and the backward all-reduces the averaged gradients in buckets while it runs
+(engine_train.py).
 """
 import os
+import zlib
 
 import torch
+import torch.distributed as dist
 
 from . import _cabi as C
 from . import tc
@@ -70,18 +77,30 @@ class _Conv:
         self.shift_a = self.shift.data_ptr() if self.shift is not None else 0
 
 
+_BROADCAST_BUCKET_BYTES = 250 << 20               # DistributedDataParallel's broadcast_bucket_size
+
+
 class FusedMinkUNet:
-    def __init__(self, model, batch_stats=False):
+    def __init__(self, model, batch_stats=False, process_group=None):
         """model: eval-mode MinkUNet (BasicBlock variants) whose parameters live on a CUDA device.
         batch_stats=True: a train-mode model instead; every forward normalises with batch statistics and updates the BatchNorm
-        running buffers in place, as ``model(sinput)`` in train mode under no_grad does."""
+        running buffers in place, as ``model(sinput)`` in train mode under no_grad does.
+        process_group (batch_stats only): train data-parallel over this group as ``DistributedDataParallel(model)`` does;
+        every rank must build its engine, run the same number of forwards and backwards, and pass the same group."""
         net = model.net3d if hasattr(model, 'net3d') else model
         p = next(net.parameters())
         C.require_cuda(p, 'model parameters')
         self.batch_stats = bool(batch_stats)
+        if process_group is not None and not self.batch_stats:
+            raise ValueError("FusedMinkUNet: process_group needs batch_stats=True (the eval engine computes no gradients to "
+                             "all-reduce)")
         self._net = net
         self._check_mode()
         self.device = p.device
+        self.process_group = process_group
+        self._sync_buffers = True                 # DDP's require_forward_param_sync: broadcast buffers before the next forward
+        if process_group is not None:
+            self._dp_sync_module_states()         # before anything is packed from the parameters
         self.dense_up = os.environ.get('OSB_DENSE_UP', '1') != '0'
         # The packed weights and folded BatchNorm constants are COPIES: every tensor they were made from is tracked, and a
         # forward that finds one changed (load_state_dict, an optimiser step, .to()) re-packs before it runs.  With batch
@@ -105,6 +124,38 @@ class FusedMinkUNet:
         self.use_pyramid = os.environ.get('OSB_PYRAMID', '1') != '0'
         if 'OSB_TC_LAZY' in os.environ:                      # tuning: 0 = smem index prologue, 1 = lazy on >= 2-wave launches, 2 = always
             tc.debug_set_tc(lazy=int(os.environ['OSB_TC_LAZY']))
+
+    def _dp_sync_module_states(self):
+        """DistributedDataParallel's construction: refuse a model whose parameters differ in count or shape on any rank (on
+        every rank, instead of a later collective hanging), then broadcast rank 0's parameters and buffers in place."""
+        pg, net = self.process_group, self._net
+        params = list(net.parameters())
+        shapes = repr([(tuple(p.shape), str(p.dtype)) for p in params]).encode()
+        sig = torch.tensor([len(params), sum(p.numel() for p in params), zlib.crc32(shapes)], dtype=torch.int64,
+                           device=self.device)
+        got = [torch.empty_like(sig) for _ in range(dist.get_world_size(group=pg))]
+        dist.all_gather(got, sig, group=pg)
+        bad = [r for r, g in enumerate(got) if not torch.equal(g, got[0])]
+        if bad:
+            raise RuntimeError(f"FusedMinkUNet: the models of process_group ranks {bad} differ from rank 0's in parameter count "
+                               f"or shapes ({int(sig[0])} parameters on this rank, rank {dist.get_rank(group=pg)})")
+        with torch.no_grad():
+            dist._broadcast_coalesced(pg, params + list(net.buffers()), _BROADCAST_BUCKET_BYTES, 0)
+
+    def _dp_forward(self, fn, *args):
+        """fn(*args) under DistributedDataParallel's buffer rule (broadcast_buffers=True): rank 0's running buffers are
+        broadcast into every rank's storage before the first forward and before any forward that follows a grad-enabled one."""
+        if self.process_group is None:
+            return fn(*args)
+        sync_next = torch.is_grad_enabled()
+        if self._sync_buffers:
+            with torch.no_grad():
+                dist._broadcast_coalesced(self.process_group, [b for m in self._bns for b in
+                                                               (m.running_mean, m.running_var, m.num_batches_tracked)],
+                                          _BROADCAST_BUCKET_BYTES, 0)
+        out = fn(*args)
+        self._sync_buffers = sync_next
+        return out
 
     def _check_mode(self):
         if self.batch_stats:
@@ -315,11 +366,14 @@ class FusedMinkUNet:
             x = [(self._bs_norm(c2, z, n, res_a=r, res_cv=ds), c2.cout, n)]
         return x[0]
 
-    @torch.no_grad()
     def forward(self, coords, feats, coordinate_manager=None, head=None):
         """coords int32 [N,4] (batch,x,y,z), feats fp32 [N,cin], both CUDA, caller order.
         Returns fp32 [N, out_channels] in the caller's row order (== ``model(SparseTensor(feats, coords))``).
         batch_stats=True: == ``model(SparseTensor(feats, coords))`` in train mode, including the running-buffer updates."""
+        return self._dp_forward(self._forward_no_grad, coords, feats, coordinate_manager, head)
+
+    @torch.no_grad()
+    def _forward_no_grad(self, coords, feats, coordinate_manager, head):
         if not self.batch_stats:
             return self._forward(coords, feats, coordinate_manager, head)
         if head is not None:
@@ -471,7 +525,7 @@ class FusedMinkUNet:
         (bool mask or int64 caller-row index; only those rows go through the final 1x1x1 layer).  ``loss.backward()`` then
         writes / accumulates ``.grad`` of every parameter of the model.  The running buffers move once per call."""
         from . import engine_train
-        return engine_train.forward_train(self, coords, feats, rows)
+        return self._dp_forward(engine_train.forward_train, self, coords, feats, rows)
 
     def forward_train_ce(self, coords, feats, labels, ignore_index=-100):
         """Training step of a per-voxel classifier on a batch_stats engine (run/train_mink.py): returns ``(loss, pred)`` with
@@ -480,7 +534,7 @@ class FusedMinkUNet:
         trunk of width a multiple of 32 up to 384.  ``loss.backward()`` fills ``.grad`` of every parameter; the logits are
         never materialised (openscene_b200/engine_train.py, csrc/ce_head.cu)."""
         from . import engine_train
-        return engine_train.forward_train_ce(self, coords, feats, labels, ignore_index)
+        return self._dp_forward(engine_train.forward_train_ce, self, coords, feats, labels, ignore_index)
 
     # ---------------------------------------------------------------------------------------
     def fold_head(self, text_features):

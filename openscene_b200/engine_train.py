@@ -19,8 +19,17 @@ residual never alias), so two identical steps give bit-identical gradients.
 
 ``forward_train_ce`` (per-voxel classification, run/train_mink.py) runs the same trunk and replaces the final layer by
 ``osb_ce_head_fwd`` (head product, log-sum-exp, NLL over the labelled rows, argmax in caller order); its backward starts with
-``osb_ce_head_bwd``, which writes the head's weight gradient and the trunk output's gradient, and continues as above."""
+``osb_ce_head_bwd``, which writes the head's weight gradient and the trunk output's gradient, and continues as above.
+
+With a process group (``FusedMinkUNet(model, batch_stats=True, process_group=pg)``) the backward all-reduces the gradients as
+DistributedDataParallel does: the flat gradient buffer is cut at parameter boundaries into buckets, from the end of the
+parameter list (the head's and decoder's gradients are written first), of about 1 MiB for the first and 25 MiB for the others.
+Right after the tape item that writes a bucket's last slot, the bucket is divided by the world size and all-reduced
+asynchronously, ordered behind the launches already on the current stream; the backward waits on every collective (a
+stream wait for NCCL) before it returns, so the optimiser and the next forward read reduced gradients and no collective
+overlaps the next forward's launches."""
 import torch
+import torch.distributed as dist
 from torch.autograd.function import once_differentiable
 
 from . import _cabi as C
@@ -28,6 +37,8 @@ from . import tc
 from .coords import CoordinateManager
 
 _GCHUNK = 64 << 20
+_FIRST_BUCKET_BYTES = 1 << 20                     # torch.distributed._DEFAULT_FIRST_BUCKET_BYTES
+_BUCKET_BYTES = 25 << 20                          # DistributedDataParallel's bucket_cap_mb=25
 
 
 def _al(x):
@@ -398,6 +409,30 @@ def _run_forward(eng, coords, feats, rows, ce=None):
     return gr
 
 
+def plan_buckets(tape, params):
+    """[(lo, hi, t)]: all-reduce buckets over params[lo:hi], in the order the backward completes them (from the end of the
+    parameter list, DistributedDataParallel's size caps), each issued after item t of the reversed tape, the item that writes
+    the last of its slots."""
+    index = {id(p): i for i, p in enumerate(params)}
+    last = [None] * len(params)
+    for t, (kind, item) in enumerate(reversed(tape)):
+        nodes = item if kind == 'block' else (item[0] if kind == 'ce_head' else item,)
+        for nd in nodes:
+            if nd is not None:
+                bn = nd.cv.bn
+                for p in (nd.cv.mod.kernel,) + ((bn.weight, bn.bias) if bn is not None else ()):
+                    last[index[id(p)]] = t
+    if None in last:
+        raise RuntimeError(f"forward_train backward: no tape item writes the gradient of parameter {last.index(None)}")
+    out, hi, size, cap = [], len(params), 0, _FIRST_BUCKET_BYTES
+    for i in range(len(params) - 1, -1, -1):
+        size += 4 * params[i].numel()
+        if size >= cap or i == 0:
+            out.append((i, hi, max(last[i:hi])))
+            hi, size, cap = i, 0, _BUCKET_BYTES
+    return out
+
+
 def _run_backward(eng, gr, g, params):
     if gr.gen != eng._gen:
         raise RuntimeError("FusedMinkUNet: the activations saved by forward_train were overwritten by a later forward / "
@@ -409,11 +444,26 @@ def _run_backward(eng, gr, g, params):
     # one flat buffer for all parameter gradients; every slot is written by exactly one launch below
     index = {id(p): i for i, p in enumerate(params)}
     flat = torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev)
-    views, off = [], 0
+    views, offs = [], [0]
     for p in params:
-        views.append(flat[off:off + p.numel()].view(p.shape))
-        off += p.numel()
+        views.append(flat[offs[-1]:offs[-1] + p.numel()].view(p.shape))
+        offs.append(offs[-1] + p.numel())
     written = [False] * len(params)
+    pg = eng.process_group
+    buckets = plan_buckets(gr.tape, params) if pg is not None else []
+    world = dist.get_world_size(group=pg) if pg is not None else 1
+    works = []
+
+    def issue(t):
+        """all-reduce every bucket whose last slot tape item t wrote: g / world on every rank, summed"""
+        while len(works) < len(buckets) and buckets[len(works)][2] == t:
+            lo, hi, _ = buckets[len(works)]
+            if not all(written[lo:hi]):
+                raise RuntimeError(f"forward_train backward: the gradient bucket of parameters {lo}..{hi - 1} is due after "
+                                   f"tape item {t} with {hi - lo - sum(written[lo:hi])} slots still unwritten")
+            b = flat[offs[lo]:offs[hi]]
+            b.div_(world)
+            works.append(dist.all_reduce(b, group=pg, async_op=True))
 
     def slot(p):
         i = index[id(p)]
@@ -495,7 +545,7 @@ def _run_backward(eng, gr, g, params):
             grads[src] = out
 
     with torch.cuda.device(dev):
-        for kind, item in reversed(gr.tape):
+        for t, (kind, item) in enumerate(reversed(gr.tape)):
             if kind == 'head':
                 nd = item
                 cv = nd.cv
@@ -550,6 +600,10 @@ def _run_backward(eng, gr, g, params):
                     slot(cv.mod.kernel).copy_(gw[:, :cv.cin])
                 else:
                     conv_bwd(nd, dz, nd.n)
+            if buckets:
+                issue(t)
+        for w in works:
+            w.wait()
     missing = [i for i, w in enumerate(written) if not w]
     if missing:
         raise RuntimeError(f"forward_train backward: {len(missing)} parameters without a gradient")

@@ -5,8 +5,9 @@ batch index moves with x and y, which keeps scenes apart and stays below the coo
 with BatchNorm in train mode, ``CrossEntropyLoss(ignore_index=255)`` over every voxel, zero_grad / backward / optimiser step
 (SGD, momentum 0.9, weight decay 1e-4 in config/*/mink.yaml), and ``output.max(1)[1]`` for ``intersectionAndUnionGPU``."""
 import torch
-import torch.distributed as dist
 import torch.nn.functional as F
+
+from .distill import refuse_local_engine
 
 
 def _translate(coords):
@@ -33,10 +34,9 @@ def train_step(model, optimizer, coords, feats, labels, ignore_label=255, transl
 def fused_train_step(engine, optimizer, coords, feats, labels, ignore_label=255, translate=True):
     """``train_step`` on the fused engine (``FusedMinkUNet(model, batch_stats=True)``): the same random shift, loss, zero_grad,
     backward and optimiser step, with ``engine.forward_train_ce``.  Returns (loss, pred) as train_step.
-    Single process only: DistributedDataParallel wraps ``model.forward``, which the engine bypasses."""
-    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-        raise RuntimeError("fused_train_step: the fused engine does not all-reduce gradients (world size > 1); "
-                           "use train_step on the DistributedDataParallel model")
+    With more than one process, build the engine with ``process_group=dist.group.WORLD`` (distill.refuse_local_engine); the
+    loss and pred stay per rank, as in run/train_mink.py."""
+    refuse_local_engine(engine, 'fused_train_step')
     if translate:
         coords = _translate(coords)
     dev = engine.device
