@@ -473,6 +473,56 @@ int osb_aug_input_transforms(const void *coords, int32_t coords_dtype, const voi
                              int32_t batch_index, void *coords_out, void *feats_out, int32_t *item_coords,
                              float *item_feats, int64_t *item_labels, void *stream);
 
+/* ---- optimiser step and in-place weight re-pack (csrc/optim.cu) ------------------------------------------------------
+ * Multi-tensor updates: one launch over a DEVICE table of tensors, every tensor cut into chunks of chunk_elems elements
+ * (a multiple of 4); chunk_begin = the table's running sum of ceil(numel / chunk_elems), n_chunks its total.  fp32,
+ * element-wise, in the order of operations of torch.optim's foreach implementations (_multi_tensor_adam / _sgd), each
+ * rounding spelled out (DESIGN.md "Optimiser contract"):
+ *   osb_optim_adam   m = lerp(m, g, lerp_w); v = v * beta2 + one_minus_beta2 * (g * g);
+ *                    p = p + step_size * (m / (sqrt(v) / bc2_sqrt + eps))
+ *   osb_optim_sgd    d = g + weight_decay * p (weight_decay != 0); with a momentum buffer b: b = d if first else
+ *                    b * momentum + d, then d = b; p = p + neg_lr * d
+ *   osb_conv_repack  every job writes the split-bf16 operand osb_conv_pack_weights would make ([K, cout_pad, cin] rows,
+ *                    weight element (k, n, c) read at w[k sk + n sn + c sc]) into an existing buffer; chunks over
+ *                    K * cout_pad * cin packed elements per job.
+ * osb_optim_entry_bytes(kind): the size of one table entry (0 Adam, 1 SGD, 2 re-pack job; 0 for any other kind). */
+typedef struct osb_adam_tensor {
+  float *param;
+  const float *grad;
+  float *exp_avg;
+  float *exp_avg_sq;
+  int64_t numel;
+  int64_t chunk_begin;
+  float step_size;          /* -(lr / (1 - beta1^t)), in double then rounded once */
+  float bc2_sqrt;           /* (1 - beta2^t)^0.5, in double then rounded once */
+  float lerp_w;             /* 1 - beta1 */
+  float beta2;
+  float one_minus_beta2;
+  float eps;
+} osb_adam_tensor;
+typedef struct osb_sgd_tensor {
+  float *param;
+  const float *grad;
+  float *momentum_buffer;   /* NULL: momentum 0 */
+  int64_t numel;
+  int64_t chunk_begin;
+  float neg_lr;
+  float weight_decay;
+  float momentum;
+  int32_t first;            /* the buffer is new: b = d (torch's clone) */
+} osb_sgd_tensor;
+typedef struct osb_pack_job {
+  const float *w;
+  void *wpack;
+  int64_t sk, sn, sc;
+  int64_t chunk_begin;
+  int32_t K, cin, cout, cout_pad;
+} osb_pack_job;
+size_t osb_optim_entry_bytes(int32_t kind);
+int osb_optim_adam(const osb_adam_tensor *table, int32_t n_tensors, int64_t chunk_elems, int64_t n_chunks, void *stream);
+int osb_optim_sgd(const osb_sgd_tensor *table, int32_t n_tensors, int64_t chunk_elems, int64_t n_chunks, void *stream);
+int osb_conv_repack(const osb_pack_job *jobs, int32_t n_jobs, int64_t chunk_elems, int64_t n_chunks, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

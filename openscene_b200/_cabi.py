@@ -84,6 +84,10 @@ SIGNATURES = {
     'osb_aug_elastic_interp': (c_int, [P, I32, I64, P, I32, I32, I32, P, c_double, P, P]),
     'osb_aug_input_transforms': (c_int, [P, I32, P, I32, P, P, I64, P, P, P, POINTER(c_double), I32, I32, P, P, P, P, P,
                                          P]),
+    'osb_optim_entry_bytes': (SZ, [I32]),
+    'osb_optim_adam': (c_int, [P, I32, I64, I64, P]),
+    'osb_optim_sgd': (c_int, [P, I32, I64, I64, P]),
+    'osb_conv_repack': (c_int, [P, I32, I64, I64, P]),
 }
 
 

@@ -175,4 +175,21 @@ __device__ inline float join_bf16(__nv_bfloat16 hi, __nv_bfloat16 lo) {
 // byte offset of channel c (hi part) inside a split row; the lo part is +64 bytes
 __host__ __device__ inline int split_off_hi(int c) { return (c >> 5) * 128 + (c & 31) * 2; }
 
+// The split-bf16 B operand of the tensor-core convolutions (osb_conv_pack_weights, osb_conv_repack): K * cout_pad rows, row
+// kn = k * cout_pad + n holding input channels 0..cin-1 of output column n as split lines; rows n >= cout are zero.
+// Writes packed element e (channel e % cin of row e / cin); weight element (k, n, c) is read at w[k * sk + n * sn + c * sc].
+__device__ inline void pack_weight_elem(const float *__restrict__ w, int64_t sk, int64_t sn, int64_t sc, int cin, int cout,
+                                        int cout_pad, int64_t e, uint8_t *__restrict__ wpack) {
+  const int c = (int)(e % cin);
+  const int64_t kn = e / cin;
+  const int n = (int)(kn % cout_pad), k = (int)(kn / cout_pad);
+  float v = 0.f;
+  if (n < cout) v = w[k * sk + n * sn + c * sc];
+  __nv_bfloat16 hi, lo;
+  split_bf16(v, hi, lo);
+  uint8_t *row = wpack + kn * (int64_t)cin * 4 + split_off_hi(c);
+  *reinterpret_cast<__nv_bfloat16 *>(row) = hi;
+  *reinterpret_cast<__nv_bfloat16 *>(row + 64) = lo;
+}
+
 }  // namespace osb

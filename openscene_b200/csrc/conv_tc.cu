@@ -389,18 +389,9 @@ __global__ void k_conv_finish(const float *__restrict__ partial, int nsplit, int
 __global__ void k_pack_weights(const float *__restrict__ w, int K, int cin, int cout, int cout_pad, int transpose_w,
                                uint8_t *__restrict__ wpack) {
   const int64_t total = (int64_t)K * cout_pad * cin;
-  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
-    const int c = (int)(e % cin);
-    const int64_t kn = e / cin;
-    const int n = (int)(kn % cout_pad), k = (int)(kn / cout_pad);
-    float v = 0.f;
-    if (n < cout) v = transpose_w ? w[((int64_t)k * cout + n) * cin + c] : w[((int64_t)k * cin + c) * cout + n];
-    __nv_bfloat16 hi, lo;
-    split_bf16(v, hi, lo);
-    uint8_t *row = wpack + kn * (int64_t)cin * 4 + split_off_hi(c);
-    *reinterpret_cast<__nv_bfloat16 *>(row) = hi;
-    *reinterpret_cast<__nv_bfloat16 *>(row + 64) = lo;
-  }
+  const int64_t sk = (int64_t)cin * cout, sn = transpose_w ? cin : 1, sc = transpose_w ? 1 : cout;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x)
+    pack_weight_elem(w, sk, sn, sc, cin, cout, cout_pad, e, wpack);
 }
 
 // --------------------------------------------------------------------------- host side

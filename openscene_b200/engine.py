@@ -183,6 +183,35 @@ class FusedMinkUNet:
         self._tracked = list(self._net.parameters()) + ([] if self.batch_stats else list(self._net.buffers()))
         self._build()
 
+    def repack_jobs(self):
+        """Batch-statistics engine: [(weight, pack, (sk, sn, sc), K, cin, cout, cout_pad)], one ``osb_conv_repack`` job per
+        split-bf16 operand its forwards and backward read, made from the module's current weights (openscene_b200/optim.py
+        re-packs them in place after an optimiser step): the forward pack of every convolution, read as the dense-up
+        ``[1, cin, K * cout]`` matrix for the transposed ones; the final layer's pack; every per-source ``W^T`` pack the
+        backward has built so far.  The stem and the cross-entropy head multiply the parameter itself (``w3`` is the
+        parameter's storage) and the persistent-chain tiles are never read with batch statistics."""
+        if not self.batch_stats:
+            raise RuntimeError("repack_jobs: an eval-mode engine folds BatchNorm into its packs; it re-packs through refresh()")
+        jobs = []
+        for cv in (self.stem, self.final):
+            if cv.w3.data_ptr() != cv.mod.kernel.data_ptr():
+                raise RuntimeError("repack_jobs: the engine's fp32 weight copy is not the parameter's storage (refresh first)")
+        convs = [(c0, False) for (c0, _) in self.enc] + [(c0, self.dense_up) for (c0, _) in self.dec]
+        convs += [(cv, False) for (_, blocks) in self.enc + self.dec for blk in blocks for cv in blk if cv is not None]
+        convs.append((self.final, False))
+        for cv, wide in convs:
+            w = cv.mod.kernel.detach()
+            K, cin, cout = cv.K, cv.cin, cv.cout
+            if cv.wpack is not None:
+                # [K, cin, cout]: element (k, n, c) = W[k, c, n]; the dense-up pack's row k * cout + n is that same element
+                pad = cout if wide else cv.wpack.numel() // (4 * K * cin)
+                jobs.append((w, cv.wpack, (cin * cout, 1, cout), K, cin, cout, pad))
+            if isinstance(cv.bwd, list):
+                for (lo, hi, pk) in cv.bwd:                  # W[:, lo:hi, :]^T: element (k, n, c) = W[k, lo + n, c]
+                    jobs.append((w[:, lo:hi] if w.dim() == 3 else w[lo:hi], pk, (cin * cout, cout, 1), K, cout, hi - lo,
+                                 pk.numel() // (4 * K * cout)))
+        return jobs
+
     def _build(self):
         net = self._net
         fold = not self.batch_stats
