@@ -15,7 +15,8 @@
  *        own: they are arguments of osb_conv_* (scale/shift, relu, res, src1), folded into the convolution's epilogue
  *        (models/mink_unet.py:50,114,147).
  *   osb_match_*                         `predictions[inds_reverse]`, `x/(|x|+1e-5)`, `.half() @ text_features.t()`,
- *        `torch.max(pred,1)` (run/evaluate.py:288-323).
+ *        `torch.max(pred,1)` (run/evaluate.py:288-323); osb_match_ce also the cross-entropy loss and
+ *        `intersectionAndUnionGPU` of run/distill.py: validate() (:419-431) in the same pass.
  *   osb_voxelize_*                      `Voxelizer.voxelize` + `sparse_quantize`/`fnv_hash_vec`
  *        (dataset/voxelizer.py:97-140, dataset/voxelization_utils.py:9-22,44-137).
  *   osb_fusion_*                        the multi-view fusion loop: `PointCloudToImageMapper.compute_mapping`
@@ -345,6 +346,24 @@ int osb_match_ensemble_vote(const float *feat3d, const void *feat2d_f16, int64_t
  *   label_cur / label_acc as above.  1 <= K <= 512. */
 int osb_vote_accumulate(const void *src, int32_t src_is_f16, int64_t n_src, const int64_t *inds_reverse, int64_t n_pts,
                         int32_t k, void *store, int64_t *label_cur, int64_t *label_acc, void *stream);
+
+/* Validation tail of run/distill.py (:419-431) in one pass: the product of osb_match_scores with normalize = 0 (same
+ * arguments, same fp16 scores s), and for every point p with label y = label[p] (int32 or int64, label_is_i64):
+ *   logp   = fp16((s[y] - m) - log(sum_k exp(s[k] - m))) in fp32, m = max_k s[k]  (torch's CUDA log_softmax for Half)
+ *   loss   fp16 [1] = fp16(sum of -logp over rows with y != ignore_index / their number), the sum in fp64 with per-block
+ *          partials merged in a fixed order; NaN when no row is labelled (torch's `CrossEntropyLoss(ignore_index)`)
+ *   pred   int64 [n_pts] (may be NULL) = argmax_k s: the first NaN of a row if it holds one, else the first maximum
+ *   areas  in/out uint64 [3, classes] += intersection | output | target counts of (pred, y), intersectionAndUnionGPU's
+ *          rule (util/util.py:132-145): pred is ignored where y == ignore_index, values outside 0..classes-1 drop out
+ *   bad_labels  in/out int32 [1] += rows whose label lies outside [0, K) and is not ignore_index; such a row is left out
+ *          of the loss and the counts
+ *   scores_f16 (may be NULL) receives s bit-identical to osb_match_scores; otherwise s never reaches memory.
+ *   ws     8-byte aligned workspace of 16 * ceil(n_pts / 128) bytes; ws and label may be NULL when n_pts == 0
+ * 1 <= K <= 480, 1 <= classes <= 512.  Two calls on the same inputs give the same bits. */
+int osb_match_ce(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c, const int64_t *inds_reverse, int64_t n_pts,
+                 const void *text_f16, int32_t k_text, const void *label, int32_t label_is_i64, int32_t ignore_index,
+                 int32_t classes, void *scores_f16, int64_t *pred, void *loss_f16, uint64_t *areas, int32_t *bad_labels,
+                 void *ws, size_t ws_bytes, void *stream);
 
 /* Optional folded head (engine.forward_scores): rows z = [x L | x U] (fp32, row pitch ld floats) from one 1x1x1
  * convolution with the weights [L | U], W W^T = L L^T, U = W T^T  ->  score_k = fp16((x.U_k) / (|x L| + 1e-5)),

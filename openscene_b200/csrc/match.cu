@@ -8,7 +8,8 @@
 // Label rule of every non-vote kernel (k_match_scores, k_match_ensemble, k_match_tc, k_folded_head_finish): the lowest
 // column holding the largest non-NaN score, and 0 when no score is above -inf (a row of NaN and -inf only); smax is that
 // largest non-NaN score, -inf when there is none.  Labels always lie in [0, K).  torch's CUDA `max(1)[1]`, which the
-// reference takes, returns a NaN's index instead; the repeat vote follows torch's CPU rule (vote.cuh).
+// reference takes, returns a NaN's index instead; the repeat vote and the validation cross-entropy (k_match_tc_ce) follow
+// torch's CPU rule (vote.cuh).
 #include "common.cuh"
 #include <algorithm>
 #include <stdlib.h>
@@ -143,6 +144,9 @@ int match_tc_run(const void *feat, int feat_is_f16, const void *feat2_f16, const
 int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
                       const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize,
                       void *scores_f16, void *store_f16, int64_t *label_cur, int64_t *label_acc, cudaStream_t stream);
+int match_tc_ce_run(const void *feat, int feat_is_f16, int c, const int64_t *inds_reverse, int64_t n_pts, const void *text_f16,
+                    int k_text, const void *label, int label_is_i64, int ignore, int classes, void *scores_f16, int64_t *pred,
+                    void *loss_f16, uint64_t *areas, int32_t *bad, void *ws, cudaStream_t stream);
 // CUDA-core repeat vote (vote.cu)
 int vote_accumulate_run(const void *src, int src_is_f16, const int64_t *inds_reverse, int64_t n_pts, int k, void *store,
                         int64_t *label_cur, int64_t *label_acc, cudaStream_t stream);
@@ -264,6 +268,26 @@ int osb_match_ensemble_vote(const float *feat3d, const void *feat2d_f16, int64_t
   const int rc = osb_match_ensemble(feat3d, feat2d_f16, n_vox, c, inds_reverse, n_pts, smax3d, smax2d, text_f16, k_text,
                                     scratch, nullptr, nullptr, stream_);
   return match_vote_simt(rc, scratch, scores_f16 == nullptr, n_pts, k_text, store_f16, label_cur, label_acc, stream);
+}
+
+// Validation tail of run/distill.py (:419-431) in the epilogue of the tensor-core product; no CUDA-core route.
+int osb_match_ce(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c, const int64_t *inds_reverse, int64_t n_pts,
+                 const void *text_f16, int32_t k_text, const void *label, int32_t label_is_i64, int32_t ignore_index,
+                 int32_t classes, void *scores_f16, int64_t *pred, void *loss_f16, uint64_t *areas, int32_t *bad_labels,
+                 void *ws, size_t ws_bytes, void *stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  OSB_CHECK(c == 512 || c == 768, "osb_match_ce: feature width %d unsupported (OpenScene uses 512 / 768)", c);
+  OSB_CHECK(k_text >= 1 && k_text <= 480, "osb_match_ce: K_text=%d outside 1..480", k_text);
+  OSB_CHECK(classes >= 1 && classes <= 512, "osb_match_ce: classes=%d outside 1..512", classes);
+  OSB_CHECK(n_vox > 0 && n_pts >= 0, "osb_match_ce: bad shape (n_vox=%lld, n_pts=%lld)", (long long)n_vox, (long long)n_pts);
+  OSB_CHECK(label_is_i64 == 0 || label_is_i64 == 1, "osb_match_ce: label_is_i64 must be 0 or 1");
+  OSB_CHECK(feat && text_f16 && (label || n_pts == 0) && loss_f16 && areas && bad_labels,
+            "osb_match_ce: null features, text, labels, loss, areas or bad-label flag");
+  const size_t need = (size_t)16 * ceil_div(n_pts, 128);
+  OSB_CHECK(need == 0 || (ws != nullptr && ws_bytes >= need && ((uintptr_t)ws & 7) == 0),
+            "osb_match_ce: 8-byte aligned workspace of %zu bytes required (got %zu)", need, ws_bytes);
+  return match_tc_ce_run(feat, feat_is_f16, c, inds_reverse, n_pts, text_f16, k_text, label, label_is_i64, ignore_index,
+                         classes, scores_f16, pred, loss_f16, areas, bad_labels, ws, stream);
 }
 
 }  // extern "C"

@@ -17,6 +17,11 @@
 // k_match_tc_vote is the same kernel with the test-time repeat vote in the epilogue: each fp16 score is added into the
 // caller's fp16 store in place and the labels of the score row and of the summed row are kept (vote.cuh), so a repeat's
 // [N_pts, K] scores never reach HBM.  k_match_tc itself compiles to the same instructions as before the vote existed.
+//
+// k_match_tc_ce is the same kernel with the validation tail of run/distill.py in the epilogue (MatchTcCe below): the
+// cross-entropy term, the argmax and the intersection / union / target counts of every row.  k_match_tc and
+// k_match_tc_vote compile to the same instructions as before it existed.
+#include "metric.cuh"
 #include "tc_ptx.cuh"
 #include "vote.cuh"
 #include <algorithm>
@@ -52,8 +57,35 @@ struct MatchTcVote {
   int pair;                          // K even and the store 4-byte aligned: a thread's column pair is one __half2
 };
 
-template <int NP, bool VOTE>   // half2 pairs per lane: C = 64 * NP
-__device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const MatchTcParams p, const MatchTcVote vo) {
+// Validation cross-entropy (k_match_tc_ce, run/distill.py:419-431): per point row with label y, torch's CUDA log_softmax
+// for Half read at y, logp = fp16((s_y - m) - log(sum_k exp(s_k - m))) in fp32, from a running (m, sum) per row over the
+// 96-row passes; the NLL term -logp summed in fp64 (per-block partials, merged in block order by k_match_ce_loss), the
+// NaN-first argmax (vote.cuh) and util.py's intersection / union / target counts (metric.cuh).  A label outside [0, K)
+// other than ignore drops the row from the loss and the counts and is counted in *bad.
+struct MatchTcCe {
+  const void *label;                 // [n_pts] int32 or int64
+  int label_is_i64, ignore, classes;
+  double *part;                      // [gridDim.x][2]: sum of the terms, labelled rows
+  unsigned long long *areas;         // [3, classes], accumulated
+  int32_t *bad;                      // [1], accumulated
+  void *loss;                        // fp16 [1]: fp16(sum / rows), written by k_match_ce_loss
+};
+
+enum { MT_PLAIN = 0, MT_VOTE = 1, MT_CE = 2 };
+
+// the label of point row pt as an int: y in [0, K), ignore, or (a label outside [0, K)) a negative value other than ignore
+__device__ __forceinline__ int ce_label(const MatchTcCe &ce, int64_t pt, int64_t n_pts, int k_text) {
+  if (pt >= n_pts) return ce.ignore;
+  const long long y = ce.label_is_i64 ? (long long)__ldg(reinterpret_cast<const int64_t *>(ce.label) + pt)
+                                      : (long long)__ldg(reinterpret_cast<const int32_t *>(ce.label) + pt);
+  if (y == ce.ignore || (y >= 0 && y < k_text)) return (int)y;
+  return ce.ignore == -1 ? -2 : -1;
+}
+
+template <int NP, int MODE>   // half2 pairs per lane: C = 64 * NP
+__device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const MatchTcParams p, const MatchTcVote vo,
+                                              const MatchTcCe ce) {
+  constexpr bool VOTE = MODE == MT_VOTE, CE = MODE == MT_CE;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int C = 64 * NP;
@@ -73,6 +105,12 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (tid == MT_PW * 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmT) : "memory");
+  // CE: the block's 128 NLL terms and labelled-row flags, then its [3, classes] histogram
+  float *s_term = reinterpret_cast<float *>(sB + MT_BSTAGES * B_BYTES + 128);
+  int *s_lab = reinterpret_cast<int *>(s_term + MT_M);
+  uint32_t *s_hist = reinterpret_cast<uint32_t *>(s_lab + MT_M);
+  if constexpr (CE)
+    for (int b = tid; b < 3 * ce.classes; b += MT_THREADS) s_hist[b] = 0;
   __syncthreads();
   const int n_stage = p.n_pass * NP;
 
@@ -178,6 +216,13 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
     int best_k[2] = {0, 0};
     VoteArgmax vcur[2], vacc[2];
     if constexpr (VOTE) { vcur[0].init(); vcur[1].init(); vacc[0].init(); vacc[1].init(); }
+    // CE: running max / sum of exp(s - max) over this thread's columns, and the label's score (the label is re-read
+    // from L1 in every epilogue rather than held in registers across the products)
+    float lm[2], ls[2], sy[2];
+    if constexpr (CE) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) { lm[h] = -INFINITY; ls[h] = 0.f; sy[h] = 0.f; vcur[h].init(); }
+    }
     mbar_wait(a_full, 0);
     int s = 0; uint32_t phase = 0;
     for (int pass = 0; pass < p.n_pass; ++pass) {
@@ -199,9 +244,21 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
         if ((tid & 127) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(b_empty + 8 * s) : "memory");
         if (++s == MT_BSTAGES) { s = 0; phase ^= 1; }
       }
+      // CE: this pass's fp16 scores of both rows as half2 pairs (the accumulators die here)
+      __half2 hs[2][MT_NW / 8];
+      if constexpr (CE) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < MT_NW / 8; ++i) hs[h][i] = __floats2half2_rn(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int64_t pt = row0 + r_lo + 8 * h;
+        // CE: the label, then per column the score, the argmax, the pass maximum and the label's score
+        int y = 0;
+        float pm = -INFINITY;
+        if constexpr (CE) y = ce_label(ce, pt, p.n_pts, p.k_text);
 #pragma unroll
         for (int i = 0; i < MT_NW / 8; ++i) {
           if constexpr (VOTE) {
@@ -237,6 +294,19 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
                 if (two) vacc[h].take(__half2float(s1), k0 + 1);
               }
             }
+          } else if constexpr (CE) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int k = pass * MT_NW + 8 * i + cq + e;
+              if (k < p.k_text) {
+                const __half hv = e ? __high2half(hs[h][i]) : __low2half(hs[h][i]);
+                const float sc = __half2float(hv);
+                if (p.scores != nullptr && pt < p.n_pts) p.scores[pt * p.k_text + k] = hv;
+                vcur[h].take(sc, k);
+                pm = fmaxf(pm, sc);
+                if (k == y) sy[h] = sc;
+              }
+            }
           } else {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
@@ -250,6 +320,18 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
             }
           }
         }
+        if constexpr (CE) {   // the pass's exp sum against the new running maximum
+          const float mn = fmaxf(lm[h], pm), mu = mn == -INFINITY ? 0.f : mn;
+          float sum = ls[h] * expf(lm[h] - mu);
+#pragma unroll
+          for (int i = 0; i < MT_NW / 8; ++i) {
+            const float2 f = __half22float2(hs[h][i]);
+            const int k = pass * MT_NW + 8 * i + cq;
+            if (k < p.k_text) sum += expf(f.x - mu);
+            if (k + 1 < p.k_text) sum += expf(f.y - mu);
+          }
+          lm[h] = mn; ls[h] = sum;
+        }
       }
     }
     if constexpr (VOTE) {
@@ -261,6 +343,32 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
         if ((lane & 3) == 0 && pt < p.n_pts) {
           if (vo.label_cur) vo.label_cur[pt] = vcur[h].k;
           if (vo.label_acc) vo.label_acc[pt] = vacc[h].k;
+        }
+      }
+    } else if constexpr (CE) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        vcur[h].reduce<4>();
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {   // merge (max, sum) over the four lanes of the row
+          const float om = __shfl_xor_sync(0xffffffffu, lm[h], o), os = __shfl_xor_sync(0xffffffffu, ls[h], o);
+          const float mn = fmaxf(lm[h], om), mu = mn == -INFINITY ? 0.f : mn;
+          ls[h] = ls[h] * expf(lm[h] - mu) + os * expf(om - mu);
+          lm[h] = mn;
+        }
+        const int r = r_lo + 8 * h;
+        const int64_t pt = row0 + r;
+        const int y = ce_label(ce, pt, p.n_pts, p.k_text);
+        // column y belongs to lane (y % 8) / 2 of the row's quad (96 % 8 == 0)
+        const bool in_k = y >= 0 && y < p.k_text;
+        const float s_y = __shfl_sync(0xffffffffu, sy[h], (lane & ~3) | (in_k ? (y & 7) >> 1 : 0));
+        if ((lane & 3) == 0) {
+          const bool live = pt < p.n_pts, lab = live && y != ce.ignore, bad = lab && !in_k;
+          s_lab[r] = lab && in_k;
+          s_term[r] = lab && in_k ? -__half2float(__float2half_rn((s_y - lm[h]) - logf(ls[h]))) : 0.f;
+          if (bad) atomicAdd(ce.bad, 1);
+          else if (live) inter_union_add(vcur[h].k, y, ce.classes, ce.ignore, s_hist);
+          if (live && p.label) p.label[pt] = vcur[h].k;
         }
       }
     } else {
@@ -281,27 +389,78 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
       }
     }
   }
+  if constexpr (CE) {
+    __syncthreads();
+    if (warp == 0) {   // the block's partial in a fixed order: rows 4 lane .. 4 lane + 3, then a butterfly over the lanes
+      double s = 0.0, c = 0.0;
+#pragma unroll
+      for (int j = 0; j < MT_M / 32; ++j) {
+        const int r = (MT_M / 32) * lane + j;
+        if (s_lab[r]) { s += (double)s_term[r]; c += 1.0; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        s += __shfl_xor_sync(0xffffffffu, s, o);
+        c += __shfl_xor_sync(0xffffffffu, c, o);
+      }
+      if (lane == 0) { ce.part[2 * blockIdx.x] = s; ce.part[2 * blockIdx.x + 1] = c; }
+    }
+    for (int b = tid; b < 3 * ce.classes; b += MT_THREADS)
+      if (s_hist[b]) atomicAdd(&ce.areas[b], (unsigned long long)s_hist[b]);
+  }
+}
+
+// one warp: the scene loss fp16(sum / rows) from the per-block partials, merged in block order (0 / 0 = NaN when no row
+// is labelled)
+__global__ void __launch_bounds__(32) k_match_ce_loss(const double *__restrict__ part, int64_t nblk, __half *loss) {
+  const int lane = threadIdx.x;
+  double s = 0.0, c = 0.0;
+  for (int64_t b = lane; b < nblk; b += 32) { s += part[2 * b]; c += part[2 * b + 1]; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, o);
+    c += __shfl_xor_sync(0xffffffffu, c, o);
+  }
+  if (lane == 0) *loss = __double2half(s / c);
 }
 
 template <int NP>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
-  match_tc_body<NP, false>(tmT, p, MatchTcVote{});
+  match_tc_body<NP, MT_PLAIN>(tmT, p, MatchTcVote{}, MatchTcCe{});
 }
 
 template <int NP>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 k_match_tc_vote(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, const MatchTcVote vo) {
-  match_tc_body<NP, true>(tmT, p, vo);
+  match_tc_body<NP, MT_VOTE>(tmT, p, vo, MatchTcCe{});
 }
 
-static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, const void *text_f16, cudaStream_t stream) {
+template <int NP>
+__global__ void __launch_bounds__(MT_THREADS, 1)
+k_match_tc_ce(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, const MatchTcCe ce) {
+  match_tc_body<NP, MT_CE>(tmT, p, MatchTcVote{}, ce);
+}
+
+static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, const MatchTcCe *ce, const void *text_f16,
+                           cudaStream_t stream) {
   CUtensorMap tmT;
   if (make_tmap_2b(&tmT, text_f16, (uint64_t)p.C, (uint64_t)p.k_text, MT_NW, 1)) return 1;
   const int NP = p.C / 64;
   const size_t smem = (size_t)NP * MT_M * 128 + MT_BSTAGES * MT_NW * 128 + 128 + 1024;
   const unsigned grid = (unsigned)ceil_div(p.n_pts, MT_M);
-  if (vote != nullptr) {
+  if (ce != nullptr) {
+    const size_t smem_ce = smem + 2 * MT_M * 4 + (size_t)3 * ce->classes * 4;   // + terms, flags, histogram
+    if (NP == 12) {
+      OSB_SMEM_ATTR_ONCE(k_match_tc_ce<12>, 227 * 1024);
+      k_match_tc_ce<12><<<grid, MT_THREADS, smem_ce, stream>>>(tmT, p, *ce);
+    } else {
+      OSB_SMEM_ATTR_ONCE(k_match_tc_ce<8>, 227 * 1024);
+      k_match_tc_ce<8><<<grid, MT_THREADS, smem_ce, stream>>>(tmT, p, *ce);
+    }
+    OSB_LAUNCH_CHECK();
+    k_match_ce_loss<<<1, 32, 0, stream>>>(ce->part, grid, (__half *)ce->loss);
+  } else if (vote != nullptr) {
     if (NP == 12) {
       OSB_SMEM_ATTR_ONCE(k_match_tc_vote<12>, 227 * 1024);
       k_match_tc_vote<12><<<grid, MT_THREADS, smem, stream>>>(tmT, p, *vote);
@@ -340,7 +499,7 @@ int match_tc_run(const void *feat, int feat_is_f16, const void *feat2_f16, const
   if (fill_match_tc(p, feat, feat_is_f16, feat2_f16, sel_a, sel_b, c, inds_reverse, n_pts, k_text, normalize, scores_f16,
                     label, smax, feat_out_f16))
     return 1;
-  return launch_match_tc(p, nullptr, text_f16, stream);
+  return launch_match_tc(p, nullptr, nullptr, text_f16, stream);
 }
 
 int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
@@ -352,7 +511,23 @@ int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, 
     return 1;
   const MatchTcVote vote{(__half *)store_f16, label_cur, label_acc,
                          (k_text % 2 == 0 && reinterpret_cast<uintptr_t>(store_f16) % 4 == 0) ? 1 : 0};
-  return launch_match_tc(p, &vote, text_f16, stream);
+  return launch_match_tc(p, &vote, nullptr, text_f16, stream);
+}
+
+int match_tc_ce_run(const void *feat, int feat_is_f16, int c, const int64_t *inds_reverse, int64_t n_pts, const void *text_f16,
+                    int k_text, const void *label, int label_is_i64, int ignore, int classes, void *scores_f16, int64_t *pred,
+                    void *loss_f16, uint64_t *areas, int32_t *bad, void *ws, cudaStream_t stream) {
+  if (n_pts == 0) {   // no row: NaN loss, nothing counted
+    k_match_ce_loss<<<1, 32, 0, stream>>>(nullptr, 0, (__half *)loss_f16);
+    OSB_LAUNCH_CHECK();
+    return 0;
+  }
+  MatchTcParams p;
+  if (fill_match_tc(p, feat, feat_is_f16, nullptr, nullptr, nullptr, c, inds_reverse, n_pts, k_text, 0, scores_f16, pred,
+                    nullptr, nullptr))
+    return 1;
+  const MatchTcCe ce{label, label_is_i64, ignore, classes, (double *)ws, (unsigned long long *)areas, bad, loss_f16};
+  return launch_match_tc(p, nullptr, &ce, text_f16, stream);
 }
 
 }  // namespace osb

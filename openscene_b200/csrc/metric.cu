@@ -2,6 +2,7 @@
 // and the intersection / union / target histograms of util/util.py:132-145 (which round-trips through .cpu() for
 // torch.histc).  Integer counting: per-block shared-memory histograms, flushed with 64-bit atomics.
 #include "common.cuh"
+#include "metric.cuh"
 
 #include <algorithm>
 
@@ -44,19 +45,9 @@ k_inter_union(const T *__restrict__ out, const T *__restrict__ tgt, int64_t n, i
     __syncthreads();
   }
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const long long t = (long long)tgt[i];
-    long long o = (long long)out[i];
-    if (t == ignore_id) o = ignore_id;                   // util.py:138 output[target == ignore_index] = ignore_index
-    const bool o_in = o >= 0 && o < K, t_in = t >= 0 && t < K;     // histc(bins=K, min=0, max=K-1) drops the rest
-    if (use_smem) {
-      if (o_in && o == t) atomicAdd(&s_bins[(int)o], 1u);
-      if (o_in) atomicAdd(&s_bins[K + (int)o], 1u);
-      if (t_in) atomicAdd(&s_bins[2 * K + (int)t], 1u);
-    } else {
-      if (o_in && o == t) atomicAdd(&areas[o], 1ull);
-      if (o_in) atomicAdd(&areas[K + o], 1ull);
-      if (t_in) atomicAdd(&areas[2 * K + t], 1ull);
-    }
+    const long long t = (long long)tgt[i], o = (long long)out[i];
+    if (use_smem) inter_union_add(o, t, K, ignore_id, s_bins);
+    else inter_union_add(o, t, K, ignore_id, areas);
   }
   if (use_smem) {
     __syncthreads();

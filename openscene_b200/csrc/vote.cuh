@@ -1,4 +1,5 @@
-// Running argmax of the test-time repeat vote (csrc/vote.cu, the vote epilogue of csrc/match_tc.cu).
+// Running argmax of the test-time repeat vote (csrc/vote.cu, the vote epilogue of csrc/match_tc.cu) and of the validation
+// cross-entropy epilogue (k_match_tc_ce).
 //
 // The evaluation drivers take labels with torch's CPU `x.float().max(1)[1]` (run/evaluate.py:400, run/eval_mink.py:205):
 // a row holding a NaN takes the index of its first NaN; otherwise the first maximum wins (-0 == +0, ties go to the lowest
