@@ -136,6 +136,12 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) {
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
+// no ordering of later accesses behind it: the thread stalls only where the value is used
+__device__ __forceinline__ unsigned ld_relaxed_u32(const unsigned *p) {
+  unsigned v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
+  return v;
+}
 
 // Sense-reversing grid barrier over {count, generation} in global memory (both zero before the first use ever; the
 // barrier leaves count == 0 behind, so no host-side reset between launches).  Every CTA of the grid must be resident:
@@ -331,11 +337,16 @@ k_conv_chain(const __grid_constant__ ChainArgs args, int n_layers, unsigned *gba
     for (int s = 0; s < sb; ++s) { mbar_init(fullB + 8 * s, 1); mbar_init(emptyB + 8 * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  unsigned bar_gen = 0;
-  if (tid == 0 && gbar) bar_gen = ld_acquire_u32(gbar + 1);    // before this launch's first barrier can complete
   __syncthreads();
   // Everything above touched no data of an earlier kernel in the stream; from here on we read activations.
+  // PDL pre-wait reads: none (the layer descriptors are launch parameters)
   if (flags & 1) asm volatile("griddepcontrol.wait;" ::: "memory");
+  // The barrier generation is read behind the wait: the previous chain launch in the stream may still be running its own
+  // barriers until then (a grid smaller than the SM count lets this launch's CTAs start beside it), and a generation read
+  // too early lets this launch's barriers pass without waiting.  It is read before this launch's first barrier can complete;
+  // the wait has made the previous launches' last value visible, so a relaxed load suffices and costs no stall before use.
+  unsigned bar_gen = 0;
+  if (tid == 0 && gbar) bar_gen = ld_relaxed_u32(gbar + 1);
   if (dbg_clock && tid == 0) dbg_clock[blockIdx.x * 32 + 1] = clock64();
 
   // pipeline state of this thread's role; persists over items and layers

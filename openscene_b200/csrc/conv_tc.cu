@@ -131,6 +131,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   __syncthreads();
   // Everything above touched only launch-invariant data (kernel map, BN constants).  The activations, the residual
   // and the shared split workspace belong to the previous kernel in the stream: wait for it to finish and flush.
+  // PDL pre-wait reads: nbr[K][n_out], scale[cout], shift[cout]
   if (p.pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
   const uint32_t kmask = (p.dbg_skip & 4) ? 0u : (p.lazy_idx ? (p.K >= 32 ? 0xffffffffu : ((1u << p.K) - 1u)) : s_misc[0]);
   if (p.dbg_clock && tid == 0) p.dbg_clock[blockIdx.x * 8 + 1] = clock64();
@@ -340,6 +341,7 @@ __global__ void k_conv_finish(const float *__restrict__ partial, int nsplit, int
                               float *__restrict__ out_f32, const int32_t *__restrict__ out_row_map, int pdl) {
   if (pdl) {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    // PDL pre-wait reads: none
     asm volatile("griddepcontrol.wait;" ::: "memory");           // partials come from the k_conv_tc launch just before
   }
   const int groups = cout / 8;
