@@ -300,6 +300,26 @@ int osb_ce_head_fwd(const void *x_split, int64_t n, int32_t cin, const float *w,
 int osb_ce_head_bwd(const void *x_split, int64_t n, int32_t cin, const float *w, int32_t C, const int32_t *row_map,
                     const void *labels, int32_t labels_are_i64, int64_t ignore_index, const float *lse, const float *g,
                     const int64_t *n_valid, void *dx_split, float *dw, void *ws, size_t ws_bytes, void *stream);
+/* Evaluation head over points (FusedMinkUNet.forward_eval_ce; run/train_mink.py's validate() after the forward): the same
+ * row pass as osb_ce_head_fwd, walking points instead of rows.  Point p reads split row row_map[inds_reverse[p]]
+ * (row_map[p] when inds_reverse is NULL, then n_pts == n_rows) and its label at p:
+ *   row_map      int32 [n_rows]: internal row of caller row v (the coordinate manager's inv_perm)
+ *   inds_reverse int64 [n_pts] caller row of every point, values in [0, n_rows), or NULL (may be NULL when n_pts == 0)
+ *   labels       int32 or int64 [n_pts] (labels_are_i64); may be NULL when n_pts == 0
+ *   loss         fp32 [1] = sum of lse - z[label] over points with a label in [0, C) / their number (fp64 sum, per-block
+ *                partials merged in a fixed order); NaN when no point is labelled or n_pts == 0 (torch's 0 / 0)
+ *   pred         int64 [n_pts] (may be NULL) = first argmax of z (the first NaN of a row if it holds one)
+ *   areas        in/out uint64 [3, C] += intersection | output | target counts of (pred, label), intersectionAndUnionGPU's
+ *                rule (util/util.py:132-145): pred is ignored where label == ignore_index, values outside 0..C-1 drop out
+ *   bad_labels   in/out int32 [1] += points whose label lies outside [0, C) and is not ignore_index; such a point is left
+ *                out of the loss and the counts
+ *   ws           osb_ce_head_eval_workspace_bytes(n_pts, cin, C) bytes, 256-byte aligned (0 for shapes the call rejects)
+ * Shapes as osb_ce_head_fwd.  No host synchronisation; two calls on the same inputs give the same bits. */
+size_t osb_ce_head_eval_workspace_bytes(int64_t n_pts, int32_t cin, int32_t C);
+int osb_ce_head_eval(const void *x_split, int64_t n_rows, int32_t cin, const float *w, int32_t C, const int32_t *row_map,
+                     const int64_t *inds_reverse, int64_t n_pts, const void *labels, int32_t labels_are_i64,
+                     int32_t ignore_index, int64_t *pred, float *loss, uint64_t *areas, int32_t *bad_labels, void *ws,
+                     size_t ws_bytes, void *stream);
 
 /* fp32 [n,c] <-> split rows. */
 int osb_f32_to_split(const float *in, int64_t n, int32_t c, void *out_split, void *stream);

@@ -6,6 +6,9 @@
 //                    loss = sum of nll over labelled rows / n_valid (fp64 sum, per-block partials merged in a fixed order).
 //   osb_ce_head_bwd  d = (softmax(z) - onehot(label)) g / n_valid on labelled rows (0 elsewhere), dx = d W^T (split rows),
 //                    dW = sum_r x_r^T d_r (fp32 per-split partials, merged in fp64 in a fixed order).
+//   osb_ce_head_eval the forward row pass over points (run/train_mink.py's validate()): point p reads the row of its voxel,
+//                    loss as above over labelled points, pred[p], intersection / union / target counts (metric.cuh) and
+//                    a count of labels outside [0, C); no lse, no logits.
 //
 // Why CUDA cores and not wgmma: for cin = 96, C = 20 a row is 384 B of split bf16 and 2 * 96 * 20 = 3.8 kFLOP of product
 // (forward), ~10 FLOP per HBM byte, below the H100's fp32 ridge (67 TFLOP/s over 3.35 TB/s = 20 FLOP/B).  The head is bound
@@ -26,6 +29,7 @@
 //
 // Row-to-block assignment and every merge order are functions of n only: two calls give identical bits.
 #include "common.cuh"
+#include "metric.cuh"
 #include <algorithm>
 #include <math.h>
 
@@ -71,6 +75,18 @@ static size_t ce_ws_layout(int64_t n, int cin, int c, void *base, CeWs *out) {
   return a + b + d + e;
 }
 
+// evaluation workspace: W_pad [cin][cp] | loss partials [row blocks of n_pts][2] fp64 | labelled points int64 [1]
+static size_t ce_eval_ws_layout(int64_t n_pts, int cin, int c, void *base, CeWs *out, int64_t **n_valid) {
+  const size_t a = al256((size_t)cin * ce_cpad(c) * sizeof(float));
+  const size_t b = al256((size_t)ce_row_blocks(n_pts) * 2 * sizeof(double));
+  if (out) {
+    uint8_t *p = (uint8_t *)base;
+    *out = CeWs{(float *)p, (double *)(p + a), nullptr, nullptr};
+    *n_valid = (int64_t *)(p + a + b);
+  }
+  return a + b + 256;
+}
+
 __global__ void k_ce_pad_w(const float *__restrict__ w, int cin, int c, int cp, float *__restrict__ wp) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cin * cp; i += gridDim.x * blockDim.x) {
     const int k = i / cp, j = i - k * cp;
@@ -113,29 +129,52 @@ __device__ inline void ce_chunk_logits(const uint8_t *row, int cin, const float 
   }
 }
 
-// forward row pass: lse, pred (caller order), per-block (sum of nll, labelled rows)
-template <typename L>
-__global__ void __launch_bounds__(CE_THREADS) k_ce_fwd(const uint8_t *__restrict__ x, int64_t n, int cin,
-                                                          const float *__restrict__ wp, int c, int cp,
-                                                          const int32_t *__restrict__ row_map, const L *__restrict__ labels,
-                                                          long long ignore, float *__restrict__ lse, int64_t *__restrict__ pred,
-                                                          double *__restrict__ part) {
+// Evaluation variant of the forward row pass (k_ce_fwd_eval): the pass walks points instead of rows.  Point p reads split
+// row row_map[inds_reverse[p]] (row_map[p] without inds_reverse) and its label at p; it writes pred[p] (if pred is set), adds
+// its NLL term to the block partial when it is labelled, and counts (pred, label) into the block's shared histogram
+// (metric.cuh, intersectionAndUnionGPU's rule), flushed with 64-bit atomics.  A label outside [0, C) other than the ignore
+// label leaves the point out of the loss and the counts and is counted in *bad.
+struct CeEval {
+  const int64_t *inds_reverse;       // NULL: one point per caller row
+  uint32_t *hist;                    // shared [3, C]
+  unsigned long long *areas;         // [3, C] += intersection | output | target
+  int32_t *bad;                      // += points with a label outside [0, C) other than the ignore label
+};
+
+// the row pass of k_ce_fwd (EVAL = false: rows in internal order, labels and pred in caller order) and of k_ce_fwd_eval
+template <typename L, bool EVAL>
+__device__ __forceinline__ void ce_fwd_rows(const uint8_t *__restrict__ x, int64_t n, int cin, const float *__restrict__ wp,
+                                            int c, int cp, const int32_t *__restrict__ row_map, const L *__restrict__ labels,
+                                            long long ignore, float *__restrict__ lse, int64_t *__restrict__ pred,
+                                            double *__restrict__ part, const CeEval ev) {
   __shared__ double s_sum[CE_THREADS / 32], s_cnt[CE_THREADS / 32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t row_bytes = (int64_t)cin * 4;
+  if constexpr (EVAL) {
+    for (int b = threadIdx.x; b < 3 * c; b += CE_THREADS) ev.hist[b] = 0;
+    __syncthreads();
+  }
   double sum = 0.0, cnt = 0.0;
   for (int64_t grp = (int64_t)blockIdx.x * (CE_THREADS / 32) + warp; grp * 32 < n; grp += (int64_t)gridDim.x * (CE_THREADS / 32)) {
     const int64_t r = grp * 32 + lane;
     const bool valid = r < n;
     const int64_t rr = valid ? r : n - 1;
-    const int32_t cr = __ldg(row_map + rr);
-    const long long lab = (long long)__ldg(labels + cr);
+    int64_t xr = rr;
+    int32_t cr = 0;
+    long long lab;
+    if constexpr (EVAL) {
+      xr = __ldg(row_map + (ev.inds_reverse ? __ldg(ev.inds_reverse + rr) : rr));
+      lab = (long long)__ldg(labels + rr);
+    } else {
+      cr = __ldg(row_map + rr);
+      lab = (long long)__ldg(labels + cr);
+    }
     float m = -INFINITY, s = 0.f, best = -INFINITY, zl = 0.f;
     int arg = 0;
     bool found = false;
     for (int j = 0; j < cp / 32; ++j) {
       float z[32];
-      ce_chunk_logits(x + rr * row_bytes, cin, wp, cp, j, z);
+      ce_chunk_logits(x + xr * row_bytes, cin, wp, cp, j, z);
       float mc = -INFINITY;
 #pragma unroll
       for (int q = 0; q < 32; ++q) {
@@ -156,12 +195,25 @@ __global__ void __launch_bounds__(CE_THREADS) k_ce_fwd(const uint8_t *__restrict
       m = mn;
     }
     if (valid) {
-      lse[r] = m + logf(s);
-      pred[cr] = arg;
-      if (lab != ignore) {
-        // a label outside [0, C) makes the loss NaN (the caller validates labels first)
-        sum += found ? (double)(m - zl) + log((double)s) : (double)NAN;
-        cnt += 1.0;
+      if constexpr (EVAL) {
+        if (pred) pred[r] = arg;
+        if (lab != ignore && !found) {
+          atomicAdd(ev.bad, 1);
+        } else {
+          if (lab != ignore) {
+            sum += (double)(m - zl) + log((double)s);
+            cnt += 1.0;
+          }
+          inter_union_add(arg, lab, c, (int)ignore, ev.hist);
+        }
+      } else {
+        lse[r] = m + logf(s);
+        pred[cr] = arg;
+        if (lab != ignore) {
+          // a label outside [0, C) makes the loss NaN (the caller validates labels first)
+          sum += found ? (double)(m - zl) + log((double)s) : (double)NAN;
+          cnt += 1.0;
+        }
       }
     }
   }
@@ -178,6 +230,33 @@ __global__ void __launch_bounds__(CE_THREADS) k_ce_fwd(const uint8_t *__restrict
     part[2 * blockIdx.x] = a;
     part[2 * blockIdx.x + 1] = b;
   }
+  if constexpr (EVAL)
+    for (int b = threadIdx.x; b < 3 * c; b += CE_THREADS)
+      if (ev.hist[b]) atomicAdd(&ev.areas[b], (unsigned long long)ev.hist[b]);
+}
+
+// forward row pass: lse, pred (caller order), per-block (sum of nll, labelled rows)
+template <typename L>
+__global__ void __launch_bounds__(CE_THREADS) k_ce_fwd(const uint8_t *__restrict__ x, int64_t n, int cin,
+                                                          const float *__restrict__ wp, int c, int cp,
+                                                          const int32_t *__restrict__ row_map, const L *__restrict__ labels,
+                                                          long long ignore, float *__restrict__ lse, int64_t *__restrict__ pred,
+                                                          double *__restrict__ part) {
+  ce_fwd_rows<L, false>(x, n, cin, wp, c, cp, row_map, labels, ignore, lse, pred, part, CeEval{});
+}
+
+// evaluation row pass over n_pts points: pred (may be NULL), per-block (sum of nll, labelled points), counts, bad labels
+template <typename L>
+__global__ void __launch_bounds__(CE_THREADS) k_ce_fwd_eval(const uint8_t *__restrict__ x, int64_t n_pts, int cin,
+                                                               const float *__restrict__ wp, int c, int cp,
+                                                               const int32_t *__restrict__ row_map,
+                                                               const int64_t *__restrict__ inds_reverse,
+                                                               const L *__restrict__ labels, int ignore,
+                                                               int64_t *__restrict__ pred, double *__restrict__ part,
+                                                               unsigned long long *__restrict__ areas, int32_t *__restrict__ bad) {
+  __shared__ uint32_t s_hist[3 * CE_MAX_C];
+  ce_fwd_rows<L, true>(x, n_pts, cin, wp, c, cp, row_map, labels, ignore, nullptr, pred, part,
+                       CeEval{inds_reverse, s_hist, areas, bad});
 }
 
 // one block: merge the per-block partials in a fixed order
@@ -421,6 +500,54 @@ int osb_ce_head_bwd(const void *x_split, int64_t n, int32_t cin, const float *w,
       (const uint8_t *)x_split, n, cin, s.wp, c, cp, s.d, (uint8_t *)dx_split, s.dwp);
   OSB_LAUNCH_CHECK();
   k_ce_dw_merge<<<(unsigned)ceil_div(cin * c, 256), 256, 0, stream>>>(s.dwp, splits, cin, c, cp, dw);
+  OSB_LAUNCH_CHECK();
+  return 0;
+}
+
+size_t osb_ce_head_eval_workspace_bytes(int64_t n_pts, int32_t cin, int32_t c) {
+  if (n_pts < 0 || !ce_shape_ok(1, cin, c)) return 0;
+  return ce_eval_ws_layout(n_pts, cin, c, nullptr, nullptr, nullptr);
+}
+
+int osb_ce_head_eval(const void *x_split, int64_t n_rows, int32_t cin, const float *w, int32_t c, const int32_t *row_map,
+                     const int64_t *inds_reverse, int64_t n_pts, const void *labels, int32_t labels_are_i64,
+                     int32_t ignore_index, int64_t *pred, float *loss, uint64_t *areas, int32_t *bad_labels, void *ws,
+                     size_t ws_bytes, void *stream_) {
+  const char *fn = "osb_ce_head_eval";
+  OSB_CHECK(n_rows >= 1, "%s: rows (%lld) must be positive", fn, (long long)n_rows);
+  OSB_CHECK(n_pts >= 0, "%s: points (%lld) must not be negative", fn, (long long)n_pts);
+  OSB_CHECK(inds_reverse || n_pts == n_rows || n_pts == 0, "%s: without inds_reverse every row is one point (%lld points, %lld rows)", fn,
+            (long long)n_pts, (long long)n_rows);
+  OSB_CHECK(cin >= 32 && cin <= CE_MAX_CIN && cin % 32 == 0, "%s: input channels (%d) must be a multiple of 32 up to %d", fn, cin,
+            CE_MAX_CIN);
+  OSB_CHECK(c >= 1 && c <= CE_MAX_C, "%s: classes (%d) must be 1 to %d", fn, c, CE_MAX_C);
+  OSB_CHECK(x_split && w && row_map && (labels || n_pts == 0), "%s: null rows, weights, row map or labels", fn);
+  OSB_CHECK(loss && areas && bad_labels, "%s: null loss, areas or bad-label count", fn);
+  OSB_CHECK(labels_are_i64 == 0 || labels_are_i64 == 1, "%s: labels_are_i64 must be 0 or 1", fn);
+  OSB_CHECK(((uintptr_t)x_split & 15) == 0, "%s: rows must be 16-byte aligned", fn);
+  const size_t need = ce_eval_ws_layout(n_pts, cin, c, nullptr, nullptr, nullptr);
+  OSB_CHECK(ws != nullptr && ws_bytes >= need && ((uintptr_t)ws & 255) == 0,
+            "%s: 256-byte aligned workspace of %zu bytes required (got %zu)", fn, need, ws_bytes);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  CeWs s;
+  int64_t *n_valid;
+  ce_eval_ws_layout(n_pts, cin, c, ws, &s, &n_valid);
+  const int cp = ce_cpad(c);
+  const int64_t nblk = ce_row_blocks(n_pts);
+  if (n_pts > 0) {
+    k_ce_pad_w<<<(unsigned)ceil_div(cin * cp, 256), 256, 0, stream>>>(w, cin, c, cp, s.wp);
+    OSB_LAUNCH_CHECK();
+    if (labels_are_i64)
+      k_ce_fwd_eval<int64_t><<<(unsigned)nblk, CE_THREADS, 0, stream>>>(
+          (const uint8_t *)x_split, n_pts, cin, s.wp, c, cp, row_map, inds_reverse, (const int64_t *)labels, ignore_index, pred,
+          s.part, (unsigned long long *)areas, bad_labels);
+    else
+      k_ce_fwd_eval<int32_t><<<(unsigned)nblk, CE_THREADS, 0, stream>>>(
+          (const uint8_t *)x_split, n_pts, cin, s.wp, c, cp, row_map, inds_reverse, (const int32_t *)labels, ignore_index, pred,
+          s.part, (unsigned long long *)areas, bad_labels);
+    OSB_LAUNCH_CHECK();
+  }
+  k_ce_loss<<<1, CE_THREADS, 0, stream>>>(s.part, nblk, loss, n_valid);     // no point: 0 / 0 = NaN
   OSB_LAUNCH_CHECK();
   return 0;
 }

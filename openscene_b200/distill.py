@@ -227,9 +227,10 @@ class DeviceValidation:
         return validation_result(self._loss[:n], self._areas[:n], self._bad[:n], weight, self.process_group)
 
 
-def validation_result(losses, areas, bad, weight=1, process_group=None):
-    """DeviceValidation.end on its per-scene state (any device): ``losses`` fp16 [n], ``areas`` int64 [n, 3, classes]
-    (intersection, output, target), ``bad`` int32 [n] counts of labels outside [0, K) other than the ignore label."""
+def validation_result(losses, areas, bad, weight=1, process_group=None, owner='DeviceValidation'):
+    """DeviceValidation.end (and train_mink.DeviceMinkValidation.end, ``owner`` naming it in errors) on its per-scene state
+    (any device): ``losses`` fp16 or fp32 [n], ``areas`` int64 [n, 3, classes] (intersection, output, target), ``bad`` int32
+    [n] counts of labels outside [0, K) other than the ignore label."""
     import numpy as np
     n = losses.shape[0]
     bad = bad.cpu()
@@ -240,14 +241,14 @@ def validation_result(losses, areas, bad, weight=1, process_group=None):
         dist.all_reduce(st, op=dist.ReduceOp.MAX, group=process_group)
         hi, lo, any_bad = int(st[0]), -int(st[1]), int(st[2])
         if hi != lo:
-            raise RuntimeError(f"DeviceValidation.end: the ranks added between {lo} and {hi} scenes (this rank {n}); "
+            raise RuntimeError(f"{owner}.end: the ranks added between {lo} and {hi} scenes (this rank {n}); "
                                f"every rank must validate the same number of scenes")
         if any_bad and not bool(bad.any()):
-            raise IndexError("DeviceValidation.end: another rank saw labels outside [0, K) other than the ignore label")
+            raise IndexError(f"{owner}.end: another rank saw labels outside [0, K) other than the ignore label")
     hit = torch.nonzero(bad).view(-1)
     if hit.numel():
         s = int(hit[0])
-        raise IndexError(f"DeviceValidation.end: scene {s} (0-based, in add() order) has {int(bad[s])} labels outside "
+        raise IndexError(f"{owner}.end: scene {s} (0-based, in add() order) has {int(bad[s])} labels outside "
                          f"[0, K) other than the ignore label")
     if world > 1:
         areas = areas.cpu() if on_cpu else areas.clone()

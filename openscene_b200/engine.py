@@ -109,7 +109,7 @@ class FusedMinkUNet:
         self._bs_ws = None
         self._gen = 0                             # bumped by every forward: a training graph whose activations were overwritten
         self._garena = []                         # training: grow-only chunks of gradient rows (engine_train.py)
-        self._ce_ws = None                        # training: workspace of the cross-entropy head (engine_train.py)
+        self._ce_ws = None                        # workspace of the cross-entropy heads (engine_train.py, forward_eval_ce)
         self._build()
         self.out_channels = self.final.cout
         self.last_cm = None
@@ -418,7 +418,9 @@ class FusedMinkUNet:
                 # in-place updates do, so that an eval-mode engine or fast_eval on this model re-folds them
                 torch.autograd.graph.increment_version(self._bs_tensors)
 
-    def _forward(self, coords, feats, coordinate_manager, head):
+    def _forward(self, coords, feats, coordinate_manager, head, tail=None):
+        """The trunk, then the folded ``head``, the caller's ``tail(cur, n0, cm)`` on the last activation (split rows in
+        internal order; its result is returned) or, with neither, the final layer."""
         C.require_cuda(feats, 'features')
         if self._sig != self._signature():                     # the source module changed since the weights were packed
             self.refresh()
@@ -525,6 +527,9 @@ class FusedMinkUNet:
                 if bs:
                     self._bs_norm(uconv, y, n[l])
                 cur = self._stage(blocks, [(y, uconv.cout, n[l]), skips[l]], nbr3_a[l], n[l])
+            if tail is not None:
+                self._chain_run()
+                return tail(cur, n[0], cm)
             if head is not None:                           # folded head: 96 -> (96 + K) conv, rows straight in caller order
                 z = torch.empty((n[0], head.cout), dtype=torch.float32, device=self.device)
                 self._conv(head, [cur], 0, n[0], relu=0, out_f32_a=z.data_ptr(), row_map_a=cm.perm.data_ptr())
@@ -564,6 +569,56 @@ class FusedMinkUNet:
         never materialised (openscene_b200/engine_train.py, csrc/ce_head.cu)."""
         from . import engine_train
         return self._dp_forward(engine_train.forward_train_ce, self, coords, feats, labels, ignore_index)
+
+    @torch.no_grad()
+    def forward_eval_ce(self, coords, feats, labels, inds_reverse, loss, areas, bad, ignore_index=255, pred=None):
+        """Validation tail of a per-voxel classifier on the eval engine (run/train_mink.py's validate() after
+        ``output = model(sinput)``): the trunk runs as in ``forward``, and one launch (osb_ce_head_eval) replaces the final
+        layer, the ``output[inds_reverse]`` gather, ``CrossEntropyLoss(ignore_index)``, ``output.max(1)[1]`` and
+        ``intersectionAndUnionGPU``; the logits are never written.  No host synchronisation.
+
+        labels: int32 / int64 [n_pts] per point; inds_reverse: int64 [n_pts] voxel (caller row) of every point, or None (one
+        point per row).  Outputs, device tensors the caller owns: ``loss`` fp32 (first element) = the loss over points with
+        a label in [0, C) (NaN when there is none), ``areas`` int64 [3, C] += intersection | output | target counts, ``bad``
+        int32 (first element) += points whose label is outside [0, C) and not ``ignore_index`` (left out of the loss and the
+        counts), ``pred`` (optional) int64 [n_pts] = the first argmax per point."""
+        from .engine_train import CE_CIN, CE_MAX_CLASSES
+        if self.batch_stats:
+            raise NotImplementedError("forward_eval_ce: an eval-mode engine (FusedMinkUNet without batch_stats) folds BatchNorm "
+                                      "into the trunk; validate on FusedMinkUNet(model.eval())")
+        fin = self.final
+        if fin.cout > CE_MAX_CLASSES or fin.cin not in CE_CIN or fin.K != 1:
+            raise NotImplementedError(f"forward_eval_ce: a 1x1x1 head of {fin.cin} -> {fin.cout} channels (supported: input "
+                                      f"width a multiple of 32 up to 384, 1 to {CE_MAX_CLASSES} classes)")
+        dev = self.device
+        n_rows = feats.shape[0]
+        inv = None if inds_reverse is None else inds_reverse.to(dev, torch.int64, non_blocking=True).contiguous().view(-1)
+        n_pts = n_rows if inv is None else inv.numel()
+        lab = torch.as_tensor(labels).to(dev, non_blocking=True).contiguous().view(-1)
+        if lab.dtype not in (torch.int32, torch.int64):
+            lab = lab.long()
+        if lab.numel() != n_pts:
+            raise ValueError(f"forward_eval_ce: {lab.numel()} labels for {n_pts} points")
+        for t, what, dt, k in ((loss, 'loss', torch.float32, 1), (areas, 'areas', torch.int64, 3 * fin.cout),
+                               (bad, 'bad', torch.int32, 1), (pred, 'pred', torch.int64, n_pts)):
+            if t is None and what == 'pred':
+                continue
+            if t.device != dev or t.dtype != dt or not t.is_contiguous() or t.numel() < k:
+                raise ValueError(f"forward_eval_ce: {what} must be a contiguous {dt} tensor of at least {k} elements on {dev}")
+
+        def tail(cur, n0, cm):
+            fin = self.final                                # _forward re-packs (a new final) when the weights changed
+            need = C.lib().osb_ce_head_eval_workspace_bytes(n_pts, cur[1], fin.cout)
+            if self._ce_ws is None or self._ce_ws.numel() < need:
+                self._ce_ws = None
+                self._ce_ws = torch.empty(max(need, 256), dtype=torch.uint8, device=dev)
+            rc = C.lib().osb_ce_head_eval(cur[0], n0, cur[1], fin.w3.data_ptr(), fin.cout, cm.inv_perm.data_ptr(),
+                                          C.ptr(inv), n_pts, lab.data_ptr(), int(lab.dtype == torch.int64), int(ignore_index),
+                                          C.ptr(pred), loss.data_ptr(), areas.data_ptr(), bad.data_ptr(), self._ce_ws.data_ptr(),
+                                          self._ce_ws.numel(), self._stream)
+            if rc:
+                C.check(rc, 'osb_ce_head_eval')
+        self._forward(coords, feats, None, None, tail)
 
     # ---------------------------------------------------------------------------------------
     def fold_head(self, text_features):
