@@ -321,6 +321,29 @@ int osb_ce_head_eval(const void *x_split, int64_t n_rows, int32_t cin, const flo
                      int32_t ignore_index, int64_t *pred, float *loss, uint64_t *areas, int32_t *bad_labels, void *ws,
                      size_t ws_bytes, void *stream);
 
+/* Cosine distillation head on split rows (FusedMinkUNet.forward_train_cosine; run/distill.py's loss_type 'cosine'): the final
+ * 1x1x1 layer f = x w, then loss = mean over the m supervised rows of 1 - CosineSimilarity(dim=1, eps=1e-8)(f, t).  The
+ * C-wide rows f and their gradient are never written.
+ *   x_split  split rows [n, cin] (internal order); cin a multiple of 32 up to 384, C 512 or 768 (other shapes are refused)
+ *   w        fp32 [cin, C], 16-byte aligned
+ *   rows     int32 [m], 1 <= m <= n: internal row of every supervised row, caller order, distinct (dx is written, not added)
+ *   target   fp16 [m, C] in the order of rows, 16-byte aligned; widened to fp32 exactly
+ *   state    fp64 [m, 3] = (|f|, f.t, |t|) per supervised row, written by the forward and read by the backward
+ *   ws       osb_cos_head_workspace_bytes(m, cin, C) bytes, 256-byte aligned (0 for shapes the calls reject)
+ * osb_cos_head_fwd: f = x w (fp32, k ascending), the row sums in fp64; loss (fp32 [1]) = sum_r (1 - f.t / (max(|f|, eps)
+ *   max(|t|, eps))) / m, the sum in fp64 with per-block partials merged in a fixed order.
+ * osb_cos_head_bwd: with g (fp32 [1], the upstream gradient of loss) read on the device (no host sync), dloss/df_r =
+ *   a_r t_r + b_r f_r with a_r = -g / (m n1c n2c), b_r = g (f.t) / (m n1c^2 n2c |f|) (0 when |f| = 0), n1c = max(|f|, eps),
+ *   n2c = max(|t|, eps) (torch's clamps, without gradient); dx_split [n, cin] = dloss/df_r w^T at rows[r] and exactly 0 on
+ *   every other row; dw (fp32 [cin, C], overwritten) = sum_r x_r^T dloss/df_r.  Every merge is in a fixed order: two calls
+ *   give identical bits. */
+size_t osb_cos_head_workspace_bytes(int64_t m, int32_t cin, int32_t C);
+int osb_cos_head_fwd(const void *x_split, int64_t n, int32_t cin, const float *w, int32_t C, const int32_t *rows, int64_t m,
+                     const void *target, double *state, float *loss, void *ws, size_t ws_bytes, void *stream);
+int osb_cos_head_bwd(const void *x_split, int64_t n, int32_t cin, const float *w, int32_t C, const int32_t *rows, int64_t m,
+                     const void *target, const double *state, const float *g, void *dx_split, float *dw, void *ws,
+                     size_t ws_bytes, void *stream);
+
 /* fp32 [n,c] <-> split rows. */
 int osb_f32_to_split(const float *in, int64_t n, int32_t c, void *out_split, void *stream);
 int osb_split_to_f32(const void *in_split, int64_t n, int32_t c, float *out, void *stream);

@@ -58,6 +58,9 @@ SIGNATURES = {
     'osb_ce_head_bwd': (c_int, [P, I64, I32, P, I32, P, P, I32, I64, P, P, P, P, P, P, SZ, P]),
     'osb_ce_head_eval_workspace_bytes': (SZ, [I64, I32, I32]),
     'osb_ce_head_eval': (c_int, [P, I64, I32, P, I32, P, P, I64, P, I32, I32, P, P, P, P, P, SZ, P]),
+    'osb_cos_head_workspace_bytes': (SZ, [I64, I32, I32]),
+    'osb_cos_head_fwd': (c_int, [P, I64, I32, P, I32, P, I64, P, P, P, P, SZ, P]),
+    'osb_cos_head_bwd': (c_int, [P, I64, I32, P, I32, P, I64, P, P, P, P, P, P, SZ, P]),
     'osb_f32_to_split': (c_int, [P, I64, I32, P, P]),
     'osb_split_to_f32': (c_int, [P, I64, I32, P, P]),
     'osb_gather_rows_f32': (c_int, [P, P, I64, I32, P, P]),

@@ -111,6 +111,24 @@ def fused_distill_step(engine, optimizer, coords, feats, feat_3d, mask, loss_typ
     return loss.detach()
 
 
+def fused_cosine_step(engine, optimizer, coords, feats, feat_3d, mask, translate=True):
+    """``fused_distill_step`` with the cosine loss on the engine's device head: the same random translation, zero_grad,
+    backward and optimiser step, with ``engine.forward_train_cosine`` in place of ``forward_train`` + ``distill_loss``, so
+    the [M, C] output rows and their gradient are never materialised.  ``feat_3d`` is cast to fp16 on the engine's device
+    (the dtype run/distill.py's targets have).  The L1 loss stays on ``fused_distill_step``."""
+    refuse_local_engine(engine, 'fused_cosine_step')
+    if translate:
+        coords = coords.clone()
+        coords[:, 1:4] += (torch.rand(3) * 100).type_as(coords)
+    dev = engine.device
+    loss = engine.forward_train_cosine(coords.to(dev, non_blocking=True), feats.to(dev, non_blocking=True),
+                                       feat_3d.to(dev, torch.float16), mask.to(dev))
+    optimizer.zero_grad()
+    loss.backward()
+    optimizer.step()
+    return loss.detach()
+
+
 def refuse_local_engine(engine, what):
     """Refuse a fused engine that keeps its gradients local when more than one process trains."""
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:

@@ -109,7 +109,7 @@ class FusedMinkUNet:
         self._bs_ws = None
         self._gen = 0                             # bumped by every forward: a training graph whose activations were overwritten
         self._garena = []                         # training: grow-only chunks of gradient rows (engine_train.py)
-        self._ce_ws = None                        # workspace of the cross-entropy heads (engine_train.py, forward_eval_ce)
+        self._ce_ws = None                        # workspace of the cross-entropy and cosine heads (engine_train.py, forward_eval_ce)
         self._build()
         self.out_channels = self.final.cout
         self.last_cm = None
@@ -569,6 +569,15 @@ class FusedMinkUNet:
         never materialised (openscene_b200/engine_train.py, csrc/ce_head.cu)."""
         from . import engine_train
         return self._dp_forward(engine_train.forward_train_ce, self, coords, feats, labels, ignore_index)
+
+    def forward_train_cosine(self, coords, feats, feat_3d, rows):
+        """Distillation step with run/distill.py's cosine loss on a batch_stats engine: returns the 0-dim fp32 loss
+        ``distill_loss(forward_train(coords, feats, rows), feat_3d)`` with a grad_fn, where ``rows`` is the bool mask or int64
+        caller-row index of the supervised rows and ``feat_3d`` their fp16 [M, C] targets in that order.  A head of 512 or 768
+        channels on a trunk of width a multiple of 32 up to 384; ``loss.backward()`` fills ``.grad`` of every parameter.  The
+        [M, C] rows and their gradient are never materialised (openscene_b200/engine_train.py, csrc/cos_head.cu)."""
+        from . import engine_train
+        return self._dp_forward(engine_train.forward_train_cosine, self, coords, feats, feat_3d, rows)
 
     @torch.no_grad()
     def forward_eval_ce(self, coords, feats, labels, inds_reverse, loss, areas, bad, ignore_index=255, pred=None):

@@ -20,6 +20,8 @@ residual never alias), so two identical steps give bit-identical gradients.
 ``forward_train_ce`` (per-voxel classification, run/train_mink.py) runs the same trunk and replaces the final layer by
 ``osb_ce_head_fwd`` (head product, log-sum-exp, NLL over the labelled rows, argmax in caller order); its backward starts with
 ``osb_ce_head_bwd``, which writes the head's weight gradient and the trunk output's gradient, and continues as above.
+``forward_train_cosine`` (distillation with run/distill.py's cosine loss) does the same with ``osb_cos_head_fwd`` (head product
+and cosine loss on the selected rows) and ``osb_cos_head_bwd``: the C-wide rows and their gradient never exist.
 
 With a process group (``FusedMinkUNet(model, batch_stats=True, process_group=pg)``) the backward all-reduces the gradients as
 DistributedDataParallel does: the flat gradient buffer is cut at parameter boundaries into buckets, from the end of the
@@ -127,8 +129,9 @@ def forward_train_ce(eng, coords, feats, labels, ignore_index=-100):
     return _CEFunction.apply(eng, coords, feats, labels, ignore_index, *params)
 
 
-def _ce_workspace(eng, n, cin, c):
-    need = C.lib().osb_ce_head_workspace_bytes(n, cin, c)
+def _ce_workspace(eng, n, cin, c, query='osb_ce_head_workspace_bytes'):
+    """the engine's head workspace (shared by the cross-entropy and cosine heads), grown to the query's size"""
+    need = getattr(C.lib(), query)(n, cin, c)
     if eng._ce_ws is None or eng._ce_ws.numel() < need:
         eng._ce_ws = None
         eng._ce_ws = torch.empty(max(need, 256), dtype=torch.uint8, device=eng.device)
@@ -184,6 +187,86 @@ class _CEFunction(torch.autograd.Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, g, _g_pred):
+        params = ctx.saved_tensors
+        grads = _run_backward(ctx.eng, ctx.graph, g, params)
+        ctx.graph = None
+        return (None, None, None, None, None) + tuple(grads)
+
+
+COS_WIDTHS = (512, 768)
+
+
+def forward_train_cosine(eng, coords, feats, feat_3d, rows):
+    """0-dim fp32 loss with a grad_fn: ``distill_loss(forward_train(coords, feats, rows), feat_3d)`` with the cosine loss.
+    The trunk runs as in forward_train; the final 1x1x1 layer and the loss are one launch (osb_cos_head_fwd) and their
+    backward another (osb_cos_head_bwd): the [M, C] rows and their gradient never exist.  feat_3d: fp16 [M, C] on the
+    engine's device, in the order of ``rows`` (bool mask or int64 caller-row index, as in forward_train)."""
+    _refuse(eng, feats)
+    C.require_cuda(feats, 'features')
+    if eng._sig != eng._signature():
+        eng.refresh()
+    fin = eng.final
+    if fin.cout not in COS_WIDTHS or fin.cin not in CE_CIN or fin.K != 1:
+        raise NotImplementedError(f"forward_train_cosine: a 1x1x1 head of {fin.cin} -> {fin.cout} channels (supported: input "
+                                  f"width a multiple of 32 up to 384, output width 512 or 768); train it with forward_train "
+                                  f"and distill_loss")
+    if not isinstance(feat_3d, torch.Tensor) or feat_3d.dtype != torch.float16:
+        raise TypeError(f"forward_train_cosine: feat_3d must be an fp16 tensor (got {getattr(feat_3d, 'dtype', type(feat_3d))})")
+    if feat_3d.dim() != 2 or feat_3d.shape[1] != fin.cout:
+        raise ValueError(f"forward_train_cosine: feat_3d of shape {tuple(feat_3d.shape)} for a head of {fin.cout} channels "
+                         f"(expected [M, {fin.cout}])")
+    if feat_3d.device != eng.device:
+        raise ValueError(f"forward_train_cosine: feat_3d is on {feat_3d.device}, the engine on {eng.device}")
+    if rows is None:
+        raise ValueError("forward_train_cosine: rows (the supervised rows) is required")
+    _ensure_bwd_packs(eng)
+    params = list(eng._net.parameters())
+    return _CosFunction.apply(eng, coords, feats, rows, feat_3d.contiguous(), *params)
+
+
+def _cos_forward(eng, cur, n0, sel, target, tape):
+    """osb_cos_head_fwd on the trunk's last activation; records what the backward reads"""
+    fin, dev = eng.final, eng.device
+    m = sel.shape[0]
+    state = torch.empty((m, 3), dtype=torch.float64, device=dev)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    ws_a, ws_b = _ce_workspace(eng, m, cur[1], fin.cout, 'osb_cos_head_workspace_bytes')
+    rc = C.lib().osb_cos_head_fwd(cur[0], n0, cur[1], fin.w3.data_ptr(), fin.cout, sel.data_ptr(), m, target.data_ptr(),
+                                  state.data_ptr(), loss.data_ptr(), ws_a, ws_b, eng._stream)
+    if rc:
+        C.check(rc, 'osb_cos_head_fwd')
+    tape.append(('cos_head', (_Node(fin, 0, 0, n0, [cur], 1, 0, 0), sel, target, state)))
+    return loss
+
+
+def _cos_backward(eng, item, g, slot, galloc, grads, stream):
+    """osb_cos_head_bwd: dW into the final kernel's gradient slot, dx = the gradient of the trunk's last activation"""
+    nd, sel, target, state = item
+    cv = nd.cv
+    (src, c, n0), = nd.srcs
+    m = sel.shape[0]
+    dx = galloc(n0 * 4 * c)
+    ws_a, ws_b = _ce_workspace(eng, m, c, cv.cout, 'osb_cos_head_workspace_bytes')
+    rc = C.lib().osb_cos_head_bwd(src, n0, c, cv.w3.data_ptr(), cv.cout, sel.data_ptr(), m, target.data_ptr(), state.data_ptr(),
+                                  g.data_ptr(), dx, slot(cv.mod.kernel).data_ptr(), ws_a, ws_b, stream)
+    if rc:
+        C.check(rc, 'osb_cos_head_bwd')
+    grads[src] = dx
+
+
+class _CosFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, eng, coords, feats, rows, target, *params):
+        graph = _run_forward(eng, coords, feats, rows, cos=target)
+        loss = graph.out
+        graph.out = None
+        ctx.eng, ctx.graph = eng, graph
+        ctx.save_for_backward(*params)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
         params = ctx.saved_tensors
         grads = _run_backward(ctx.eng, ctx.graph, g, params)
         ctx.graph = None
@@ -253,7 +336,7 @@ class _TrainFunction(torch.autograd.Function):
         return (None, None, None, None) + tuple(grads)
 
 
-def _run_forward(eng, coords, feats, rows, ce=None):
+def _run_forward(eng, coords, feats, rows, ce=None, cos=None):
     dev = eng.device
     st = eng.stem
     with torch.cuda.device(dev):
@@ -268,6 +351,8 @@ def _run_forward(eng, coords, feats, rows, ce=None):
                 raise ValueError(f"Expected more than 1 value per channel when training, got input size [{n[l]}, {c}] "
                                  f"(level {l}, tensor stride {ts[l]})")
         sel = _select(cm, rows, n[0], dev) if ce is None else None
+        if cos is not None and cos.shape[0] != sel.shape[0]:
+            raise ValueError(f"forward_train_cosine: feat_3d has {cos.shape[0]} rows for {sel.shape[0]} selected rows")
         eng._gen += 1                                    # from here on the arena is overwritten
         eng.last_cm = cm
         m3 = [cm.kernel_map(t, t, 3) for t in ts]
@@ -278,6 +363,7 @@ def _run_forward(eng, coords, feats, rows, ce=None):
         m, sel_t = n[0], None
         if ce is None:
             m = sel.shape[0]
+        if ce is None and cos is None:
             sel_t = torch.empty(n[0], dtype=torch.int32, device=dev)
             C.call('osb_kernel_map_transpose', C.ptr(sel), m, 1, C.ptr(sel_t), n[0], C.stream_ptr())
         k5 = cm.kernel_map(1, 1, st.ks)
@@ -389,7 +475,9 @@ def _run_forward(eng, coords, feats, rows, ce=None):
         if eng._cursor > end:
             raise RuntimeError("forward_train: activation arena overflow (plan_train_bytes out of date)")
         fin = eng.final
-        if ce is None:
+        if cos is not None:
+            out = _cos_forward(eng, cur, n[0], sel, cos, tape)
+        elif ce is None:
             out = torch.empty((m, fin.cout), dtype=torch.float32, device=dev)
             rc = eng._fn(cur[0], cur[1], n[0], 0, 0, 0, sel.data_ptr(), m, 1, fin.wpack_a, fin.cout, 0, 0, 0, 0, 0, out.data_ptr(),
                          0, eng._ws_a, eng._ws_bytes, eng._flags, eng._stream)
@@ -416,7 +504,7 @@ def plan_buckets(tape, params):
     index = {id(p): i for i, p in enumerate(params)}
     last = [None] * len(params)
     for t, (kind, item) in enumerate(reversed(tape)):
-        nodes = item if kind == 'block' else (item[0] if kind == 'ce_head' else item,)
+        nodes = item if kind == 'block' else (item[0] if kind in ('ce_head', 'cos_head') else item,)
         for nd in nodes:
             if nd is not None:
                 bn = nd.cv.bn
@@ -566,6 +654,8 @@ def _run_backward(eng, gr, g, params):
                 grads[src] = out
             elif kind == 'ce_head':
                 _ce_backward(eng, item, g, slot, galloc, grads, stream)
+            elif kind == 'cos_head':
+                _cos_backward(eng, item, g, slot, galloc, grads, stream)
             elif kind == 'block':
                 n1, nd_, n2 = item
                 g2 = grads[n2.y]
