@@ -14,21 +14,23 @@ workspace, the batch-statistics and cross-entropy workspaces, the gradient-row c
 the arena, which holds the saved activations, plus the weight-gradient workspaces).  The chain's grid-barrier words are
 never poisoned (their generation is carried from launch to launch); every poisoned range is checked against them.  A read
 that overtakes its producer then reads NaN, or the previous scene's rows, and every comparison is bitwise with every output
-finite.  Cases, one subprocess each:
+finite.  The cosine head's per-row state is filled with 0xFF before ``osb_cos_head_fwd`` writes it.  Cases, one subprocess
+each:
 
   * free against serialised: eval on the persistent chain and with ``OSB_CHAIN=0``, ``forward_scores`` with a folded head,
     the batch-statistics forward, ``forward_train`` + backward (row mask, all rows), ``forward_train_ce`` + backward, an Adam
-    step with its in-place re-pack followed by the next forward;
+    step with its in-place re-pack followed by the next forward, ``forward_train_cosine`` + ``(0.75 * loss).backward()``, and
+    ``distill.fused_cosine_step`` with a bound Adam followed by the next cosine loss;
   * one engine through ``tiny -> config1_50k -> tiny -> config2_200k -> config1_50k`` (eval and training) against a fresh
     engine per scene;
-  * the whole step on a side stream while the legacy default stream sleeps: work that lands on the default stream queues
-    behind the sleep and its consumer reads poison;
+  * the whole step on a side stream while the legacy default stream sleeps, with ``forward_train`` and with the cosine step
+    run/distill.py makes: work that lands on the default stream queues behind the sleep and its consumer reads poison;
   * plan switches: order-only ones (``OSB_PDL``, ``OSB_PYRAMID``, ``OSB_OCCGRID``) bitwise across settings, the others
     (``OSB_DENSE_UP``, ``OSB_CHAIN_MAX_TILES``, ``OSB_TC_LAZY``, the chain grid) free against serialised per setting;
   * the PDL window rule (tests/launch_order.py) on every free-running launch sequence.
 
-Negative controls change only the test side: the arena poisoned between forward and backward, and one mid-network
-``osb_conv_fwd_tc`` routed to the legacy stream behind the sleep."""
+Negative controls change only the test side: the arena poisoned between forward and backward, the cosine state poisoned
+between forward and backward, and one mid-network ``osb_conv_fwd_tc`` routed to the legacy stream behind the sleep."""
 import os
 import subprocess
 import sys
@@ -73,6 +75,7 @@ class Wrapper:
         self.reroute = None              # index of the osb_conv_fwd_tc call to send to the legacy stream (negative control)
         self.n_conv = 0
         self.gbars = []
+        self.cos_state = None            # (pointer, bytes) of the latest cosine head state
 
     def __getattr__(self, name):
         fn = getattr(REAL, name)
@@ -88,6 +91,9 @@ class Wrapper:
                 if p and p not in self.wg_seen:
                     self.wg_seen.add(p)
                     self.poison_raw(p, nb)
+            if name == 'osb_cos_head_fwd':
+                self.cos_state = (LO.ival(a[8]), 24 * LO.ival(a[6]))
+                self.poison_raw(*self.cos_state)
             L = LO.launch_of(name, a)
             self.seq.append(L)
             self.stats['launches'] += 1
@@ -143,6 +149,7 @@ C.call = W.call
 tc._CHAINS.clear()
 tc._PACK_CACHE.clear()
 POISON_ARENA_IN_BACKWARD = [False]
+POISON_COS_STATE_IN_BACKWARD = [False]
 
 _fwd = engine.FusedMinkUNet._forward
 
@@ -167,6 +174,8 @@ _run_backward = engine_train._run_backward
 
 def run_backward(eng, *a):
     W.poison_engine(eng, arena=POISON_ARENA_IN_BACKWARD[0])
+    if POISON_COS_STATE_IN_BACKWARD[0]:
+        W.poison_raw(*W.cos_state)
     W.bwd, W.wg_seen = True, set()
     try:
         return _run_backward(eng, *a)
@@ -190,6 +199,15 @@ def inputs(scene):
         labels[::9] = 255
         _SCENES[scene] = (coords, feats, labels, torch.randn(n, 96, device=dev, generator=g))
     return _SCENES[scene]
+
+
+def target(scene, rows):
+    """fp16 distillation targets of the rows selected by the mask rows"""
+    key = ('target', scene)
+    if key not in _SCENES:
+        g = torch.Generator(device=dev).manual_seed(2)
+        _SCENES[key] = torch.randn(rows.numel(), 768, device=dev, generator=g).half()
+    return _SCENES[key][rows]
 
 
 def make(arch, train, head=768):
@@ -250,6 +268,21 @@ def run_case(case, arch, scene, mode, eng=None, model=None):
                 out.update({f'{it} param {k}': cl(p) for k, p in model.named_parameters()})
                 y = eng.forward_train(coords, feats, rows=rows)
                 out[f'{it} next out'] = cl(y)
+        elif case == 'cos':
+            model.zero_grad(set_to_none=True)
+            loss = eng.forward_train_cosine(coords, feats, target(scene, rows), rows)
+            (0.75 * loss).backward()
+            out[f'{it} loss'] = cl(loss)
+            out.update({f'{it} {k}': v for k, v in state(model).items()})
+        elif case == 'cos_adam':
+            if it == 0:
+                opt = optim.Adam(model.parameters(), lr=1e-3)
+                opt.bind(eng)
+            loss = distill.fused_cosine_step(eng, opt, coords, feats, target(scene, rows), rows, translate=False)
+            out[f'{it} loss'] = cl(loss)
+            out.update({f'{it} {k}': v for k, v in state(model).items()})
+            out.update({f'{it} param {k}': cl(p) for k, p in model.named_parameters()})
+            out[f'{it} next loss'] = cl(eng.forward_train_cosine(coords, feats, target(scene, rows), rows))
         elif case == 'ce':
             model.zero_grad(set_to_none=True)
             loss, pred = eng.forward_train_ce(coords, feats, labels, 255)
@@ -323,9 +356,10 @@ def on_side_stream(fn, sleep=True):
     return out
 
 
-def train_step_all(arch, scene, mode):
+def train_step_all(arch, scene, mode, cos=False):
     """one training iteration as run/train_mink.py and run/distill.py make it: the voxeliser, a batch-statistics forward
-    with a device validation, forward_train + backward, an Adam step with re-pack, the next forward"""
+    with a device validation, forward_train + backward, an Adam step with re-pack, the next forward.  cos: the step
+    run/distill.py makes with the cosine loss, distill.fused_cosine_step with a bound Adam, then the next cosine loss"""
     coords, feats, labels, gout = inputs(scene)
     pts, vox = synth.scene_points('tiny')
     P = torch.from_numpy(pts).to(dev)
@@ -345,6 +379,15 @@ def train_step_all(arch, scene, mode):
         val = distill.DeviceValidation(text, 20, 255)
         val.add(y, None, labels)
         out['validation'] = torch.tensor(val.end(), dtype=torch.float64)
+        if cos:
+            rows = torch.arange(coords.shape[0], device=dev) %% 7 == 0
+            opt = optim.Adam(model.parameters(), lr=1e-3)
+            opt.bind(eng)
+            out['train loss'] = distill.fused_cosine_step(eng, opt, coords, feats, target(scene, rows), rows, translate=False)
+            out.update(state(model))
+            out.update({'param ' + k: cl(p) for k, p in model.named_parameters()})
+            out['next loss'] = cl(eng.forward_train_cosine(coords, feats, target(scene, rows), rows))
+            return out
         model.zero_grad(set_to_none=True)
         y = eng.forward_train(coords, feats, rows=None)
         y.backward(gout[:, :1].expand(-1, 768).contiguous() if y.shape[1] == 768 else gout)
@@ -390,7 +433,8 @@ def main():
         print('NEGATIVE control failed as it must: osb_conv_fwd_tc #12 on the legacy stream ->', k, 'differs', flush=True)
     elif kind == 'train':
         for case, a, sc in (('bs', arch, 'config1_50k'), ('train_mask', arch, 'config1_50k'), ('train_all', 'MinkUNet18A', 'tiny'),
-                            ('ce', 'MinkUNet18A', 'config1_50k'), ('adam', arch, 'config1_50k')):
+                            ('ce', 'MinkUNet18A', 'config1_50k'), ('adam', arch, 'config1_50k'), ('cos', arch, 'config1_50k'),
+                            ('cos_adam', arch, 'config1_50k')):
             ref = free_vs_serial(case, a, sc)
             if case == 'train_mask':
                 POISON_ARENA_IN_BACKWARD[0] = True
@@ -400,12 +444,20 @@ def main():
                 k = same(bad, ref, 'negative control', allow_nonfinite=True)
                 assert k is not None, "negative control: the arena poisoned between forward and backward was not detected"
                 print('NEGATIVE control failed as it must: arena poisoned before the backward ->', k, 'differs', flush=True)
+            if case == 'cos':
+                POISON_COS_STATE_IN_BACKWARD[0] = True
+                bad = run_case(case, a, sc, 'free')
+                POISON_COS_STATE_IN_BACKWARD[0] = False
+                W.seq = []
+                k = same(bad, ref, 'negative control', allow_nonfinite=True)
+                assert k is not None, "negative control: the cosine state poisoned between forward and backward was not detected"
+                print('NEGATIVE control failed as it must: cosine state poisoned before the backward ->', k, 'differs', flush=True)
     elif kind == 'interleave':
         order = ['tiny', 'config1_50k', 'tiny', 'config2_200k', 'config1_50k']
-        for case, a in (('eval', arch), ('train_mask', 'MinkUNet18A')):
+        for case, a in (('eval', arch), ('train_mask', 'MinkUNet18A'), ('cos', 'MinkUNet18A')):
             refs = {sc: run_case(case, a, sc, 'serial') for sc in sorted(set(order))}
             W.seq = []
-            model, eng = make(a, case != 'eval', 768 if case == 'eval' else 96)
+            model, eng = make(a, case != 'eval', 96 if case == 'train_mask' else 768)
             for sc in order:
                 got = run_case(case, a, sc, 'free', eng, model)
                 if case != 'eval':
@@ -423,6 +475,13 @@ def main():
         windows()
         must_equal(got, ref, 'training iteration on a side stream behind a sleeping default stream')
         print('OK side stream training iteration (voxeliser, batch statistics, validation, step, Adam, next forward)',
+              flush=True)
+        ref = train_step_all('MinkUNet18A', 'config1_50k', 'serial', cos=True)()
+        W.seq = []
+        got = on_side_stream(train_step_all('MinkUNet18A', 'config1_50k', 'free', cos=True))
+        windows()
+        must_equal(got, ref, 'cosine training iteration on a side stream behind a sleeping default stream')
+        print('OK side stream cosine iteration (voxeliser, batch statistics, validation, fused_cosine_step, Adam, next loss)',
               flush=True)
     elif kind == 'switches_order':
         from openscene_b200 import coords as CO

@@ -43,6 +43,7 @@ PASS = {
     'osb_bn_backward_reduce',                                                                           # test_gpu_norm_replay.py
     'osb_bn_stats_workspace_bytes',
     'osb_ce_head_fwd', 'osb_ce_head_bwd', 'osb_ce_head_workspace_bytes',                                # test_gpu_norm_replay.py
+    'osb_cos_head_fwd', 'osb_cos_head_bwd', 'osb_cos_head_workspace_bytes',                             # test_gpu_norm_replay.py
     'osb_f32_to_split', 'osb_split_to_f32', 'osb_gather_rows_f32',              # test_gpu_conv_tc.py, test_gpu_engine.py
     'osb_kernel_map_build', 'osb_kernel_map_build_grid', 'osb_kernel_map_transpose', 'osb_hash_build',  # test_gpu_coords.py
     'osb_coordset_build', 'osb_coordset_stride', 'osb_coordset_pyramid', 'osb_coordset_workspace_bytes',
@@ -363,7 +364,7 @@ class Harness:
         return self.real.osb_bn_backward_apply(*args)
 
 
-def pairing(H, model, ce):
+def pairing(H, model, head_launch):
     """each backward launch against the forward it differentiates"""
     fwd = [r for r in H.log if r['op'] == 'fwd' and not r['T']]
     dgr = [(i, r) for i, r in enumerate(H.log) if r['op'] == 'fwd' and r['T']]
@@ -374,8 +375,8 @@ def pairing(H, model, ce):
             by_mod[r['idt'][0]].append(r)
     names = [n for n, _ in H.mods]
     for mi, name in enumerate(names):
-        if ce and name == 'final':
-            continue                                   # the cross-entropy head's forward is osb_ce_head_fwd
+        if head_launch and name == 'final':
+            continue                                   # the head's forward is osb_ce_head_fwd / osb_cos_head_fwd
         assert len(by_mod[mi]) == 1, f"{name}: {len(by_mod[mi])} forward launches"
     latest, gp_bufs, n_pairs = {}, {b for b, acc in H.gp if not acc}, 0
     used = set()
@@ -415,7 +416,7 @@ def pairing(H, model, ce):
         n_pairs += 1
     # every kernel received a weight gradient: the stem's padded one, and one per source of [up | skip] inputs
     for mi, (name, k3) in enumerate(H.mods):
-        if ce and name == 'final':
+        if head_launch and name == 'final':
             continue
         grad = dict(model.named_modules())[name].kernel.grad.view(k3.shape)
         F = by_mod[mi][0]
@@ -439,7 +440,7 @@ def main():
     tc._PACK_CACHE.clear()
     tc.pack_weights = H.register(tc.pack_weights)
     tc.pack_weight_tiles = H.register(tc.pack_weight_tiles)
-    train = kind in ('train', 'train_all', 'ce')
+    train = kind in ('train', 'train_all', 'ce', 'cos')
     head = 20 if kind in ('ce', 'eval20') else 768
     model = synth.build_model(arch, head, seed=0).to(dev)
     model.train() if train else model.eval()
@@ -473,6 +474,12 @@ def main():
         loss, _ = eng.forward_train_ce(coords, feats, labels, 255)
         loss.backward()
         coverage(True)
+    elif kind == 'cos':
+        mask = torch.arange(n, device=dev) %% 7 == 0
+        feat = torch.randn(int(mask.sum()), 768, device=dev, generator=gen).half()
+        loss = eng.forward_train_cosine(coords, feats, feat, mask)
+        (0.75 * loss).backward()
+        coverage(True)
     else:
         rows = None if parts[3] == 'all' else (torch.arange(n, device=dev) %% 7 == 0)
         out = eng.forward_train(coords, feats, rows=rows)
@@ -484,7 +491,7 @@ def main():
     for op, (r, c) in sorted(H.worst.items()):
         print('WORST %%-22s err/A = %%.3f x 2^-16   (bound c = %%.1f)' %% (op, r, c), flush=True)
     if train:
-        pairs = pairing(H, model, kind == 'ce')
+        pairs = pairing(H, model, kind in ('ce', 'cos'))
         print('PAIRING', pairs, 'dgrad launches paired with their forward and weight gradient; every kernel has its wgrads;',
               'n_rs > 1 in', sum(1 for r in H.log if r['op'] == 'wgrad' and r['n_rs'] > 1), 'wgrads', flush=True)
     assert H.neg['tile'] == 1 and H.neg['stale'] == 1 and (H.neg['transpose'] == 1 or not train), dict(H.neg)
@@ -503,6 +510,8 @@ CONFIGS = [
     'train:MinkUNet34C:config1_50k:mask',
     'train:MinkUNet18A:tiny:all',
     'ce:MinkUNet18A:config1_50k',
+    'cos:MinkUNet34C:config1_50k:mask',                # the cosine distillation step: the trunk under osb_cos_head_*
+    'cos:MinkUNet18A:tiny:mask',
 ]
 ARCHS = ['MinkUNet14A', 'MinkUNet14B', 'MinkUNet14C', 'MinkUNet14D', 'MinkUNet18A', 'MinkUNet18B', 'MinkUNet18D',
          'MinkUNet34A', 'MinkUNet34B', 'MinkUNet34C']

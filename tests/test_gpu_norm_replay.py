@@ -15,10 +15,17 @@ snapshots what it wrote and compares that with tests/norm_ref.py element by elem
   earlier launch wrote, and after backward() the last dweight / dbias of each BatchNorm equal bn.weight.grad / bn.bias.grad
   bit for bit;
 * the CE head reads the trunk's last activation, final.kernel and the row permutation the input gather used, and its dW is
-  final.kernel.grad.
+  final.kernel.grad;
+* the cosine head (``forward_train_cosine``, driven with ``(0.75 * loss).backward()`` so that a dropped upstream gradient
+  shows) reads the last apply's output with its rows and width, final.kernel, the caller's targets and, as supervised rows,
+  the inverse of the input gather's permutation at the caller's mask rows in caller order; its backward reads the forward's
+  rows, weights, row index, targets and state (unchanged since the forward wrote it) and g = 0.75; its dW is
+  final.kernel.grad and its dx is the gradient the first BatchNorm backward reduce and apply read.  Both launches are compared
+  with ``cos_ref.head`` element by element.
 
-Reference-side negative controls must fail: a swapped residual form, the block's own BatchNorm on the downsample residual, and
-a dropped mask.  An entry point that is neither handled nor on the pass-through list fails the run."""
+Reference-side negative controls must fail: a swapped residual form, the block's own BatchNorm on the downsample residual, a
+dropped mask, and for the cosine head rows taken through the permutation instead of its inverse, targets rolled by one row
+and g = 1.  An entry point that is neither handled nor on the pass-through list fails the run."""
 import os
 import subprocess
 import sys
@@ -33,13 +40,14 @@ import collections, sys, torch
 sys.path.insert(0, %(root)r)
 cfg = sys.argv[1]
 from openscene_b200 import engine, synth, _cabi as C
+from tests import cos_ref as CR
 from tests import norm_ref as NR
 from tests import replay_ref as R
 
 dev = torch.device('cuda:0')
 
 PASS = {
-    'osb_bn_stats_workspace_bytes', 'osb_ce_head_workspace_bytes', 'osb_f32_to_split', 'osb_split_to_f32',
+    'osb_bn_stats_workspace_bytes', 'osb_ce_head_workspace_bytes', 'osb_cos_head_workspace_bytes', 'osb_f32_to_split', 'osb_split_to_f32',
     'osb_kernel_map_build', 'osb_kernel_map_build_grid', 'osb_kernel_map_transpose', 'osb_hash_build',
     'osb_coordset_build', 'osb_coordset_stride', 'osb_coordset_pyramid', 'osb_coordset_workspace_bytes',
     'osb_occgrid_build', 'osb_occgrid_bytes', 'osb_folded_head_finish', 'osb_conv_wgrad_tc',
@@ -50,7 +58,7 @@ PASS = {
 HANDLED = ('osb_conv_fwd_tc', 'osb_conv_desc_fill', 'osb_conv_chain_launch', 'osb_convtr_fwd_tc', 'osb_conv_stem_fused',
            'osb_conv_stem_fused_grid', 'osb_gather_rows_f32', 'osb_bn_batch_stats', 'osb_bn_batch_stats_save',
            'osb_bn_apply_split', 'osb_bn_apply_split_out', 'osb_bn_backward_reduce', 'osb_bn_backward_apply',
-           'osb_ce_head_fwd', 'osb_ce_head_bwd')
+           'osb_ce_head_fwd', 'osb_ce_head_bwd', 'osb_cos_head_fwd', 'osb_cos_head_bwd')
 
 
 def _i(a):
@@ -77,6 +85,7 @@ def rows(ptr, n, c):
 class Harness:
     def __init__(self, model):
         self.real = C.lib()
+        self.model = model
         self.bn_of = {}                                   # weight pointer -> BatchNorm name
         for name, m in model.named_modules():
             if isinstance(m, torch.nn.BatchNorm1d):
@@ -93,6 +102,9 @@ class Harness:
         self.neg = collections.Counter()
         self.gather_perm = None
         self.ce = {}
+        self.cos = {}
+        self.cos_caller = None                             # (caller rows of the mask, feat_3d, g) of a cosine step
+        self.cos_dx_readers = {}                           # BatchNorm backward entry point -> the dx it must read as g
 
     def __getattr__(self, name):
         if name in PASS:
@@ -250,7 +262,7 @@ class Harness:
             r2, t2 = NR.bn_apply(x, S['st'], res, S['st'], bool(relu))
             assert self.fails(y, r2, t2), "negative control: the block's own BatchNorm on the downsample residual passed"
             self.neg['own_bn_on_downsample'] += 1
-        self.applies.append(dict(bn=S['bn'], x=x_a, y=y_a, res=r_a, res_bn=RS['bn'] if RS else None, relu=relu))
+        self.applies.append(dict(bn=S['bn'], x=x_a, y=y_a, res=r_a, res_bn=RS['bn'] if RS else None, relu=relu, n=n, c=c))
         return 0
 
     def _bn_apply_split(self, *args):
@@ -278,6 +290,7 @@ class Harness:
         a = [_i(v) for v in args]
         y_a, g_a, z_a, n, c, mean_a, inv_a, sums_a, dw_a, db_a, acc = a[:11]
         torch.cuda.synchronize()
+        self.cos_gradient_read('osb_bn_backward_reduce', g_a)
         S = self.check_backward_operands(y_a, z_a, n, c, mean_a, inv_a)
         y, g, z = rows(y_a, n, c) if y_a else None, rows(g_a, n, c), rows(z_a, n, c)
         mean, inv, w = f32(mean_a, c), f32(inv_a, c), f32(S['w'], c)
@@ -307,6 +320,7 @@ class Harness:
         a = [_i(v) for v in args]
         y_a, g_a, z_a, n, c, mean_a, inv_a, w_a, sums_a, dz_a, gp_a, gp_acc = a[:12]
         torch.cuda.synchronize()
+        self.cos_gradient_read('osb_bn_backward_apply', g_a)
         S = self.check_backward_operands(y_a, z_a, n, c, mean_a, inv_a)
         assert w_a == S['w'], f"{S['bn']}: backward apply reads another weight"
         assert self.last_bw and self.last_bw['key'] == (y_a, g_a, z_a, sums_a), f"{S['bn']}: apply without its reduce"
@@ -383,11 +397,98 @@ class Harness:
         self.written.add(dx_a)
         return 0
 
+    # ------------------------------------------------------------ cosine head
+    def cos_within(self, got, ref):
+        for k, v in got.items():
+            r = CR.ratio(v, *ref[k])
+            assert r <= 1, f"cos-{k}: {r:.3g} of the bound"
+            self.worst['cos-' + k] = max(self.worst['cos-' + k], r)
+
+    def cos_fails(self, got, ref):
+        return any(CR.ratio(v, *ref[k]) > 1 for k, v in got.items())
+
+    def _cos_head_fwd(self, *args):
+        a = [_i(v) for v in args]
+        x_a, n, cin, w_a, c, rows_a, m, t_a, st_a, loss_a = a[:10]
+        torch.cuda.synchronize()
+        A = self.applies[-1] if self.applies else None
+        assert A is not None and (A['y'], A['n'], A['c']) == (x_a, n, cin), "the cosine head does not read the trunk's last activation"
+        assert w_a == self.model.final.kernel.data_ptr() and (cin, c) == tuple(self.model.final.kernel.shape[-2:]), \
+            "the cosine head does not read final.kernel"
+        caller, feat, _ = self.cos_caller
+        assert t_a == feat.data_ptr() and m == feat.shape[0] == caller.numel(), "the cosine head does not read the caller's targets"
+        assert self.gather_perm is not None and self.gather_perm[1] == n, "no input gather before the cosine head"
+        perm = snap(self.gather_perm[0], 4 * n).view(torch.int32).long()
+        inv = torch.empty_like(perm)
+        inv[perm] = torch.arange(n, device=dev)
+        sel = snap(rows_a, 4 * m).view(torch.int32)
+        assert torch.equal(sel.long(), inv[caller]), "the cosine head's rows are not the inverse gather permutation at the caller's rows"
+        x, w = rows(x_a, n, cin), f32(w_a, cin * c).view(cin, c)
+        t = snap(t_a, 2 * m * c).view(torch.float16).view(m, c).double()
+        rc = self.real.osb_cos_head_fwd(*args)
+        torch.cuda.synchronize()
+        if rc:
+            return rc
+        self.counts['osb_cos_head_fwd'] += 1
+        state = snap(st_a, 24 * m).view(torch.float64).view(m, 3)
+        got = dict(state=state, loss=f32(loss_a, 1)[0])
+        self.cos_within(got, CR.head(x, w, t, sel, 1.0))
+        if not self.neg['cos_rows_through_perm']:
+            assert self.cos_fails(got, CR.head(x, w, t, perm[caller], 1.0)), "negative control: rows through perm passed"
+            self.neg['cos_rows_through_perm'] += 1
+        if not self.neg['cos_targets_rolled']:
+            assert self.cos_fails(got, CR.head(x, w, t.roll(1, 0), sel, 1.0)), "negative control: rolled targets passed"
+            self.neg['cos_targets_rolled'] += 1
+        self.cos = dict(args=(x_a, n, cin, w_a, c, rows_a, m, t_a, st_a), x=x, w=w, t=t, sel=sel, state=state)
+        return 0
+
+    def _cos_head_bwd(self, *args):
+        a = [_i(v) for v in args]
+        x_a, n, cin, w_a, c, rows_a, m, t_a, st_a, g_a, dx_a, dw_a = a[:12]
+        torch.cuda.synchronize()
+        F = self.cos
+        assert F and F['args'] == (x_a, n, cin, w_a, c, rows_a, m, t_a, st_a), \
+            "the cosine backward does not read its forward's rows, weights, row index, targets and state"
+        assert torch.equal(rows(x_a, n, cin), F['x']) and torch.equal(f32(w_a, cin * c).view(cin, c), F['w']), \
+            "the cosine head's rows or weights changed between forward and backward"
+        assert torch.equal(snap(rows_a, 4 * m).view(torch.int32), F['sel'])
+        assert torch.equal(snap(t_a, 2 * m * c).view(torch.float16).view(m, c).double(), F['t'])
+        assert torch.equal(snap(st_a, 24 * m).view(torch.float64).view(m, 3).view(torch.int64), F['state'].view(torch.int64)), \
+            "the cosine state changed between forward and backward"
+        g = float(f32(g_a, 1))
+        assert g == self.cos_caller[2], f"the cosine backward reads g = {g}, not the upstream gradient {self.cos_caller[2]}"
+        rc = self.real.osb_cos_head_bwd(*args)
+        torch.cuda.synchronize()
+        if rc:
+            return rc
+        self.counts['osb_cos_head_bwd'] += 1
+        dx = rows(dx_a, n, cin)
+        r = F['sel'].long()
+        others = torch.ones(n, dtype=torch.bool, device=dev)
+        others[r] = False
+        assert bool((dx[others] == 0).all()), "the cosine dx is not 0 on the unsupervised rows"
+        dw = f32(dw_a, cin * c).view(cin, c)
+        got = dict(dx=dx[r], dW=dw)
+        self.cos_within(got, CR.head(F['x'], F['w'], F['t'], F['sel'], g))
+        if not self.neg['cos_g_one']:
+            assert self.cos_fails(got, CR.head(F['x'], F['w'], F['t'], F['sel'], 1.0)), "negative control: g = 1 passed"
+            self.neg['cos_g_one'] += 1
+        self.cos['dW'] = dw
+        self.cos_dx_readers = {'osb_bn_backward_reduce': dx_a, 'osb_bn_backward_apply': dx_a}
+        self.written.add(dx_a)
+        return 0
+
+    def cos_gradient_read(self, name, g_a):
+        """the first BatchNorm backward reduce / apply after the cosine backward reads its dx as g"""
+        want = self.cos_dx_readers.pop(name, None)
+        if want is not None:
+            assert g_a == want, f"{name}: the first BatchNorm backward does not read the cosine head's dx"
+
 
 def main():
     kind, arch, scene = cfg.split(':')[:3]
-    train = kind in ('train', 'train_all', 'ce')
-    head = 20 if kind == 'ce' else 768
+    train = kind in ('train', 'train_all', 'ce', 'cos')
+    head = 20 if kind == 'ce' else (int(cfg.split(':')[3]) if kind == 'cos' and cfg.count(':') > 2 else 768)
     model = synth.build_model(arch, head, seed=0).to(dev).train()
     H = Harness(model)
     C.lib = lambda: H
@@ -411,6 +512,15 @@ def main():
         loss, _ = eng.forward_train_ce(coords, feats, labels, 255)
         assert sorted(s['bn'] for s in H.stats) == sorted(bns), "not exactly one statistics launch per BatchNorm"
         loss.backward()
+    elif kind == 'cos':
+        caller = (torch.arange(n, device=dev) %% 7 == 0).nonzero().squeeze(1)
+        feat = torch.randn(caller.numel(), head, device=dev, generator=gen).half()
+        H.cos_caller = (caller, feat, 0.75)
+        mask = torch.zeros(n, dtype=torch.bool, device=dev)
+        mask[caller] = True
+        loss = eng.forward_train_cosine(coords, feats, feat, mask)
+        assert sorted(s['bn'] for s in H.stats) == sorted(bns), "not exactly one statistics launch per BatchNorm"
+        (0.75 * loss).backward()
     else:
         rows_ = None if cfg.endswith(':all') else (torch.arange(n, device=dev) %% 7 == 0)
         out = eng.forward_train(coords, feats, rows=rows_)
@@ -425,6 +535,11 @@ def main():
         if kind == 'ce':
             assert torch.equal(H.ce['w_val'], model.final.kernel.detach().view(H.ce['w_val'].shape))
             assert torch.equal(H.ce['dW'], model.final.kernel.grad.view(H.ce['dW'].shape)), "the CE dW is not final.kernel.grad"
+        if kind == 'cos':
+            assert H.counts['osb_cos_head_fwd'] == H.counts['osb_cos_head_bwd'] == 1, dict(H.counts)
+            assert not H.cos_dx_readers, f"no BatchNorm backward read the cosine dx: {sorted(H.cos_dx_readers)}"
+            assert torch.equal(H.cos['w'], model.final.kernel.detach().view(H.cos['w'].shape))
+            assert torch.equal(H.cos['dW'], model.final.kernel.grad.view(H.cos['dW'].shape)), "the cosine dW is not final.kernel.grad"
         print('SLOTS every BatchNorm\'s dweight / dbias equal its .grad bit for bit', flush=True)
     print('CONFIG', cfg, 'rows', n, 'BatchNorms', len(bns), flush=True)
     print('COUNTS', dict(H.counts), flush=True)
@@ -433,6 +548,8 @@ def main():
     downsample = any(A['res_bn'] for A in H.applies)
     assert H.neg['swapped_form'] == H.neg['own_bn_on_downsample'] == (1 if downsample else 0), dict(H.neg)
     assert H.neg['dropped_mask'] == (1 if train else 0), dict(H.neg)
+    cos_neg = [H.neg[k] for k in ('cos_rows_through_perm', 'cos_targets_rolled', 'cos_g_one')]
+    assert cos_neg == [1 if kind == 'cos' else 0] * 3, dict(H.neg)
     print('NEGATIVE controls failed as they must:', dict(H.neg), flush=True)
     print('OK')
 
@@ -446,6 +563,8 @@ CONFIGS = [
     'train:MinkUNet18A:config1_50k:mask',
     'train:MinkUNet18A:config1_50k:all',
     'ce:MinkUNet18A:config1_50k',
+    'cos:MinkUNet34C:config1_50k',                     # the shipped distillation step: 768-wide head on 96 channels
+    'cos:MinkUNet14D:config1_50k:512',                 # cin 384: the head's largest shared-memory plan
 ]
 ARCHS = ['MinkUNet14A', 'MinkUNet14B', 'MinkUNet14C', 'MinkUNet14D', 'MinkUNet18A', 'MinkUNet18B', 'MinkUNet18D',
          'MinkUNet34A', 'MinkUNet34B', 'MinkUNet34C']
@@ -465,3 +584,8 @@ def test_norm_replay(cfg):
 @pytest.mark.parametrize('arch', ARCHS)
 def test_norm_replay_every_architecture(arch):
     _run(f'train_all:{arch}:tiny:mask')
+
+
+@pytest.mark.parametrize('arch', ARCHS)
+def test_norm_replay_cosine_every_architecture(arch):
+    _run(f'cos:{arch}:tiny')

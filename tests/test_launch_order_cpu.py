@@ -4,8 +4,8 @@ The engine's Python runs on CPU tensors with the device entry points recorded (t
 and tests/test_engine_train_plan_cpu.py), here with one more layer that keeps every recorded call in stream order and with
 kernel maps the size the kernels read.  For every launch with the PDL attribute, what it reads before ``griddepcontrol.wait``
 (``k_conv_tc``: its kernel-map rows and BatchNorm scale / shift) must not be written by any launch of its PDL window: the
-eval forward on the persistent chain and on one launch per layer, and the training forward and backward, for all ten
-architectures and three scene sizes.  The table of pre-wait reads is checked against the comments the kernels carry next to
+eval forward on the persistent chain and on one launch per layer, the training forward and backward, and the cosine
+distillation step (``forward_train_cosine`` and its backward), for all ten architectures and three scene sizes.  The table of pre-wait reads is checked against the comments the kernels carry next to
 their waits.  Negative controls: the persistent chain's former read of its grid-barrier generation before the wait, and a
 kernel map produced inside the window of the layer that reads it."""
 import pytest
@@ -14,6 +14,7 @@ import torch
 from openscene_b200 import _cabi as C
 from openscene_b200 import engine, engine_train, minkunet, synth
 from tests import launch_order as LO
+from tests import test_engine_train_plan_cpu as tp
 from tests.test_engine_plan_cpu import SCENES, _FakeCM
 from tests.test_engine_plan_cpu import recorded as eval_recorded        # noqa: F401 (fixture)
 from tests.test_engine_train_plan_cpu import recorded as train_recorded  # noqa: F401 (fixture)
@@ -121,6 +122,31 @@ def test_train_plan_respects_pdl_windows(train_recorded, monkeypatch, arch, scen
     heads = [L for L in seq if L.name == 'osb_conv_fwd_tc' and L.pdl and L.operands['nbr']
              and L.operands['nbr'][0][1] - L.operands['nbr'][0][0] == 4 * int(rows.sum())]
     assert len(heads) == 2
+
+
+@pytest.mark.parametrize('scene', list(SCENES))
+@pytest.mark.parametrize('arch', sorted(minkunet.ARCHS))
+def test_cosine_plan_respects_pdl_windows(train_recorded, monkeypatch, arch, scene):  # noqa: F811
+    assert LO.is_host_only('osb_cos_head_workspace_bytes')
+    monkeypatch.setattr(tp, '_HOST', tp._HOST | {'osb_cos_head_workspace_bytes'})
+    n = train_recorded.n = SCENES[scene]
+    monkeypatch.setattr(engine_train, 'CoordinateManager', lambda coords, pyramid_levels=0: _SizedCM(n))
+    seq = _in_order(monkeypatch)
+    model = synth.build_model(arch, 768, seed=0).train()
+    eng = engine.FusedMinkUNet(model, batch_stats=True)
+    rows = torch.arange(n[0]) % 7 == 0
+    target = torch.ones(int(rows.sum()), 768, dtype=torch.float16)
+    for _ in range(2):
+        model.zero_grad(set_to_none=True)
+        loss = eng.forward_train_cosine(torch.zeros(n[0], 4, dtype=torch.int32), torch.ones(n[0], 3), target, rows)
+        (0.75 * loss).backward()
+    s = _summary(seq)
+    assert not s['bad'], s['bad'][:3]
+    assert s['pdl'] > 0 and s['windows'] == s['pdl']
+    # the head is two plain launches per step, each closing the window of what follows it; no tensor-core head launch
+    heads = [L for L in seq if L.name in ('osb_cos_head_fwd', 'osb_cos_head_bwd')]
+    assert [L.name for L in heads] == ['osb_cos_head_fwd', 'osb_cos_head_bwd'] * 2 and not any(L.pdl or L.triggers for L in heads)
+    assert not any(L.name == 'osb_conv_fwd_tc' and L.writes and any(w[2] == 'out_f32' for w in L.writes) for L in seq)
 
 
 def test_prewait_table_matches_the_kernels():
