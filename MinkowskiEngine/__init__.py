@@ -5,7 +5,8 @@ run/distill.py:18 and run/evaluate.py:18 resolves here when this repository is o
 """
 from openscene_b200.me import *  # noqa: F401,F403
 from openscene_b200.me import (CoordinateMapKey, MinkowskiAvgPooling, MinkowskiBatchNorm, MinkowskiConvolution,
-                               MinkowskiConvolutionTranspose, MinkowskiGlobalMaxPooling, MinkowskiLinear,
-                               MinkowskiReLU, MinkowskiSumPooling, SparseTensor, __version__, cat)
+                               MinkowskiConvolutionTranspose, MinkowskiGlobalAvgPooling, MinkowskiGlobalMaxPooling,
+                               MinkowskiGlobalSumPooling, MinkowskiLinear, MinkowskiMaxPooling, MinkowskiReLU,
+                               MinkowskiSumPooling, SparseTensor, __version__, cat)
 from openscene_b200.coords import CoordinateManager  # noqa: F401
 from . import modules, utils  # noqa: F401

@@ -585,6 +585,32 @@ int osb_optim_adam(const osb_adam_tensor *table, int32_t n_tensors, int64_t chun
 int osb_optim_sgd(const osb_sgd_tensor *table, int32_t n_tensors, int64_t chunk_elems, int64_t n_chunks, void *stream);
 int osb_conv_repack(const osb_pack_job *jobs, int32_t n_jobs, int64_t chunk_elems, int64_t n_chunks, void *stream);
 
+/* ------------------------------------------------------------------ pooling (fp32, CUDA cores)
+ * `MinkowskiSumPooling` / `MinkowskiAvgPooling` / `MinkowskiMaxPooling` (models/resnet_base.py:54) and the global poolings
+ * (:68).  mode: 0 sum, 1 avg, 2 max.  No atomics: two runs give the same bits.
+ *   osb_pool_fwd   out[o] over the present offsets k of nbr[K][n_out] (input row nbr[k][o], -1 none), ascending k:
+ *                  sum = fp32 adds from +0.0; avg = sum / fp32(max(count, 1)) and count[o] (int32) written;
+ *                  max = the largest input, first NaN wins, ties (+-0 equal) to the lowest k, 0 when no offset is present;
+ *                  argk[o, c] (uint16) = the winning k, 0xFFFF for none.  1 <= K <= 65535.
+ *   osb_pool_bwd   on the transposed map nbr_t[K][n_in]: gin[i] = fp32 adds over ascending k of, with o = nbr_t[k][i]:
+ *                  g[o] (sum), fp32(g[o] / max(count[o], 1)) (avg), g[o, c] where argk[o, c] == k (max).
+ *   osb_global_pool_fwd  out[b, c] over the rows r with batch[r] == b, rows in the caller's order, 1 <= n_batch:
+ *                  sum / avg: fp64 partials per chunk of rows, merged in chunk order and rounded to fp32 once (avg divides
+ *                  by the row count in fp64 first; count[b] written); an empty batch gives 0 (sum) or NaN (avg);
+ *                  max: exact, first NaN wins, ties to the lowest row, argrow[b, c] = the winning row; empty: -inf, -1.
+ *                  The workspace (osb_global_pool_workspace_bytes, 16-byte aligned) is overwritten.
+ *   osb_global_pool_bwd  gin[r] = g[batch[r]] (sum), fp32(g[b] / count[b]) (avg), g[b, c] on the winning row else 0 (max).
+ * count is needed for avg, argk / argrow for max; both are ignored (may be NULL) in the other modes. */
+int osb_pool_fwd(const float *in, int32_t c, const int32_t *nbr, int64_t n_out, int32_t K, int32_t mode, float *out,
+                 int32_t *count, uint16_t *argk, void *stream);
+int osb_pool_bwd(const float *gout, int32_t c, const int32_t *nbr_t, int64_t n_in, int32_t K, int32_t mode,
+                 const int32_t *count, const uint16_t *argk, float *gin, void *stream);
+size_t osb_global_pool_workspace_bytes(int64_t n, int32_t c, int32_t n_batch);
+int osb_global_pool_fwd(const float *in, const int32_t *batch, int64_t n, int32_t c, int32_t n_batch, int32_t mode,
+                        float *out, int32_t *count, int32_t *argrow, void *ws, size_t ws_bytes, void *stream);
+int osb_global_pool_bwd(const float *gout, const int32_t *batch, int64_t n, int32_t c, int32_t mode, const int32_t *count,
+                        const int32_t *argrow, float *gin, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -94,6 +94,11 @@ SIGNATURES = {
     'osb_optim_adam': (c_int, [P, I32, I64, I64, P]),
     'osb_optim_sgd': (c_int, [P, I32, I64, I64, P]),
     'osb_conv_repack': (c_int, [P, I32, I64, I64, P]),
+    'osb_pool_fwd': (c_int, [P, I32, P, I64, I32, I32, P, P, P, P]),
+    'osb_pool_bwd': (c_int, [P, I32, P, I64, I32, I32, P, P, P, P]),
+    'osb_global_pool_workspace_bytes': (SZ, [I64, I32, I32]),
+    'osb_global_pool_fwd': (c_int, [P, P, I64, I32, I32, I32, P, P, P, P, SZ, P]),
+    'osb_global_pool_bwd': (c_int, [P, P, I64, I32, I32, P, P, P, P]),
 }
 
 

@@ -208,6 +208,16 @@ class CoordinateManager:
             self.kmaps[key] = km
         return km
 
+    def batch_index(self, ts):
+        """(int32 batch index of every row in ``.F`` order, batch count = largest index + 1) of the set at ts.  The count
+        is read from the device once per set and cached."""
+        cache = self.__dict__.setdefault('_batch_index', {})
+        hit = cache.get(ts)
+        if hit is None:
+            b = self.coords_external(ts)[:, 0].contiguous()
+            hit = cache[ts] = (b, int(b.max().item()) + 1)
+        return hit
+
     def coords_external(self, ts):
         """int32 [N,4] in the caller's row order (stride 1) / internal order (coarser sets)."""
         c = self.sets[ts].coords

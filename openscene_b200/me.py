@@ -465,55 +465,163 @@ class MinkowskiReLU(nn.Module):
 
 
 class MinkowskiLinear(nn.Module):
+    """``nn.Linear`` on the feature matrix.  A dense ``[B, C]`` tensor (what the global poolings return here) gives a dense
+    tensor back, so ``final(glob_avg(x))`` of models/resnet_base.py:118-119 runs; a SparseTensor gives a SparseTensor."""
     _osb_me_op = True      # an operator of this package (fast_eval.py looks for the module that CALLS them)
     def __init__(self, in_features, out_features, bias=True):
         super().__init__()
         self.linear = nn.Linear(in_features, out_features, bias=bias)
 
     def forward(self, input):
+        if isinstance(input, torch.Tensor):
+            return self.linear(input)
         return SparseTensor._wrap(self.linear(input._F), input.coordinate_manager, input._ts)
+
+
+# ------------------------------------------------------------------------------------------------
+# pooling (csrc/pool.cu; the rules are DESIGN.md's "Pooling contract")
+# ------------------------------------------------------------------------------------------------
+POOL_SUM, POOL_AVG, POOL_MAX = 0, 1, 2
+
+
+class SparsePoolFunction(torch.autograd.Function):
+    """Sum / average / max over the kernel map ``kmap`` (nbr[K][n_out]); the backward walks ``kmap.transposed()``.
+    Average pooling keeps the per-output count and max pooling the winning offset per (row, channel) for the backward."""
+
+    @staticmethod
+    def forward(ctx, x, kmap, mode):
+        _require_f32(x, 'pooling input')
+        if kmap.K > 65535:
+            raise ValueError(f"openscene_b200: pooling supports kernel volumes up to 65535, got {kmap.K}")
+        if x.shape[0] != kmap.n_in:
+            raise ValueError(f"pooling input has {x.shape[0]} rows, its coordinate set has {kmap.n_in}")
+        x = x.contiguous()
+        c, n_out, dev = x.shape[1], kmap.n_out, x.device
+        out = torch.empty((n_out, c), dtype=torch.float32, device=dev)
+        count = torch.empty(n_out, dtype=torch.int32, device=dev) if mode == POOL_AVG else None
+        argk = torch.empty((n_out, c), dtype=torch.int16, device=dev) if mode == POOL_MAX else None   # uint16 bits
+        with torch.cuda.device(dev):
+            C.call('osb_pool_fwd', C.ptr(x), c, C.ptr(kmap.nbr), n_out, kmap.K, mode, C.ptr(out), C.ptr(count),
+                   C.ptr(argk), C.stream_ptr())
+        ctx.kmap, ctx.mode = kmap, mode
+        ctx.save_for_backward(count if mode == POOL_AVG else argk)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        _require_f32(g, 'pooling output gradient')
+        (aux,) = ctx.saved_tensors
+        g = g.contiguous()
+        kt = ctx.kmap.transposed()
+        gin = torch.empty((kt.n_out, g.shape[1]), dtype=torch.float32, device=g.device)
+        count = aux if ctx.mode == POOL_AVG else None
+        argk = aux if ctx.mode == POOL_MAX else None
+        with torch.cuda.device(g.device):
+            C.call('osb_pool_bwd', C.ptr(g), g.shape[1], C.ptr(kt.nbr), kt.n_out, kt.K, ctx.mode, C.ptr(count),
+                   C.ptr(argk), C.ptr(gin), C.stream_ptr())
+        return gin, None, None
+
+
+class GlobalPoolFunction(torch.autograd.Function):
+    """Sum / average / max of the rows of ``x`` per batch index ``batch`` (int32, one per row) -> dense [n_batch, C]."""
+
+    @staticmethod
+    def forward(ctx, x, batch, n_batch, mode):
+        _require_f32(x, 'global pooling input')
+        x = x.contiguous()
+        n, c, dev = x.shape[0], x.shape[1], x.device
+        out = torch.empty((n_batch, c), dtype=torch.float32, device=dev)
+        count = torch.empty(n_batch, dtype=torch.int32, device=dev) if mode == POOL_AVG else None
+        argrow = torch.empty((n_batch, c), dtype=torch.int32, device=dev) if mode == POOL_MAX else None
+        ws_bytes = C.lib().osb_global_pool_workspace_bytes(n, c, n_batch)
+        with torch.cuda.device(dev):
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+            C.call('osb_global_pool_fwd', C.ptr(x), C.ptr(batch), n, c, n_batch, mode, C.ptr(out), C.ptr(count),
+                   C.ptr(argrow), C.ptr(ws), ws_bytes, C.stream_ptr())
+        ctx.mode, ctx.n = mode, n
+        ctx.save_for_backward(batch, count if mode == POOL_AVG else argrow)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        _require_f32(g, 'global pooling output gradient')
+        batch, aux = ctx.saved_tensors
+        g = g.contiguous()
+        gin = torch.empty((ctx.n, g.shape[1]), dtype=torch.float32, device=g.device)
+        count = aux if ctx.mode == POOL_AVG else None
+        argrow = aux if ctx.mode == POOL_MAX else None
+        with torch.cuda.device(g.device):
+            C.call('osb_global_pool_bwd', C.ptr(g), C.ptr(batch), ctx.n, g.shape[1], ctx.mode, C.ptr(count), C.ptr(argrow),
+                   C.ptr(gin), C.stream_ptr())
+        return gin, None, None, None
 
 
 class _PoolBase(nn.Module):
     _osb_me_op = True      # an operator of this package (fast_eval.py looks for the module that CALLS them)
+    MODE = None
+
     def __init__(self, kernel_size, stride=1, dilation=1, kernel_generator=None, dimension=None):
         super().__init__()
         if dimension != 3:
             raise NotImplementedError("dimension=3 only")
-        self.kernel_size, self.stride, self.dilation = kernel_size, stride, dilation
+        if kernel_generator is not None:
+            raise NotImplementedError("custom kernel generators are not implemented")
+        for name, v in (('kernel_size', kernel_size), ('stride', stride), ('dilation', dilation)):
+            if not isinstance(v, int) and len(set(v)) != 1:
+                raise NotImplementedError(f"anisotropic {name} is not implemented")
+        self.kernel_size = kernel_size if isinstance(kernel_size, int) else kernel_size[0]
+        self.stride = stride if isinstance(stride, int) else stride[0]
+        self.dilation = dilation if isinstance(dilation, int) else dilation[0]
 
-    def _sum(self, input, with_count):
+    def forward(self, input):
         cm, ts = input.coordinate_manager, input._ts
         ts_out = cm.stride(ts, self.stride) if self.stride > 1 else ts
         kmap = cm.kernel_map(ts, ts_out, self.kernel_size, self.dilation)
-        c = input._F.shape[1]
-        # pooling == convolution with K identity kernels; done channel-block-diagonally by the f32 conv
-        eye = torch.eye(c, device=input._F.device).unsqueeze(0).expand(kmap.K, c, c).contiguous()
-        s = SparseConvFunction.apply(input._F, eye, kmap, kmap.n_out)
-        cnt = (kmap.nbr >= 0).sum(0).clamp(min=1).to(s.dtype).unsqueeze(1) if with_count else None
-        return s, cnt, ts_out
+        return SparseTensor._wrap(SparsePoolFunction.apply(input._F, kmap, self.MODE), cm, ts_out)
+
+    def __repr__(self):
+        return (f"{self.__class__.__name__}(kernel_size=[{self.kernel_size}]*3, stride=[{self.stride}]*3, "
+                f"dilation=[{self.dilation}]*3)")
 
 
 class MinkowskiSumPooling(_PoolBase):
-    def forward(self, input):
-        s, _, ts_out = self._sum(input, False)
-        return SparseTensor._wrap(s, input.coordinate_manager, ts_out)
+    """Sum over the inputs present in the window (fp32 adds in offset order)."""
+    MODE = POOL_SUM
 
 
 class MinkowskiAvgPooling(_PoolBase):
-    def forward(self, input):
-        s, cnt, ts_out = self._sum(input, True)
-        return SparseTensor._wrap(s / cnt, input.coordinate_manager, ts_out)
+    """Sum over the present inputs divided by their count (an output with none gives 0)."""
+    MODE = POOL_AVG
 
 
-class MinkowskiGlobalMaxPooling(nn.Module):
+class MinkowskiMaxPooling(_PoolBase):
+    """Per channel the largest present input: the first NaN in offset order wins, ties go to the lowest offset and an output
+    with no present input gives 0 and receives no gradient."""
+    MODE = POOL_MAX
+
+
+class _GlobalPoolBase(nn.Module):
+    """Pooling over all rows of each batch index, in ``.F`` row order.  Returns the dense ``[B, C]`` matrix with
+    ``B = max batch index + 1`` (MinkowskiEngine returns a SparseTensor whose ``.F`` is this matrix); a batch index without
+    rows gives 0 (sum), NaN (average) or -inf (max)."""
     _osb_me_op = True      # an operator of this package (fast_eval.py looks for the module that CALLS them)
+    MODE = None
+
     def __init__(self, dimension=None, **kw):
         super().__init__()
 
     def forward(self, input):
-        b = input.coordinate_manager.sets[input._ts].coords[:, 0].long()
-        nb = int(b.max().item()) + 1
-        out = torch.full((nb, input._F.shape[1]), float('-inf'), device=input._F.device)
-        out = out.scatter_reduce(0, b.unsqueeze(1).expand_as(input._F), input._F, reduce='amax')
-        return out
+        batch, n_batch = input.coordinate_manager.batch_index(input._ts)
+        return GlobalPoolFunction.apply(input.F, batch, n_batch, self.MODE)
+
+
+class MinkowskiGlobalSumPooling(_GlobalPoolBase):
+    MODE = POOL_SUM
+
+
+class MinkowskiGlobalAvgPooling(_GlobalPoolBase):
+    MODE = POOL_AVG
+
+
+class MinkowskiGlobalMaxPooling(_GlobalPoolBase):
+    MODE = POOL_MAX
