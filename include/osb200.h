@@ -344,6 +344,29 @@ int osb_cos_head_bwd(const void *x_split, int64_t n, int32_t cin, const float *w
                      const void *target, const double *state, const float *g, void *dx_split, float *dw, void *ws,
                      size_t ws_bytes, void *stream);
 
+/* L1 distillation head on split rows (FusedMinkUNet.forward_train_l1; run/distill.py's loss_type 'l1'): the final 1x1x1 layer
+ * f = x w, then loss = torch.nn.L1Loss()(f, t), the mean of |f - t| over the m x C elements.  The C-wide rows f and their
+ * gradient are never written.
+ *   x_split  split rows [n, cin] (internal order); cin a multiple of 32 up to 384, C 512 or 768 (other shapes are refused)
+ *   w        fp32 [cin, C], 16-byte aligned
+ *   rows     int32 [m], 1 <= m <= n: internal row of every supervised row, caller order, distinct (dx is written, not added)
+ *   target   fp16 [m, C] in the order of rows, 16-byte aligned; widened to fp32 exactly
+ *   signs    uint32 [m, C / 16], 16-byte aligned: sign(f - t) of every element, 2 bits each (element j of a row in bits
+ *            2 (j % 16) .. 2 (j % 16) + 1 of word j / 16; 0: d = +-0 or NaN, 1: +1, 2: -1), written by the forward and
+ *            the only per-row state the backward reads
+ *   ws       osb_l1_head_workspace_bytes(m, cin, C) bytes, 256-byte aligned (0 for shapes the calls reject)
+ * osb_l1_head_fwd: f = x w (fp32, k ascending), d = fp32(f - t); loss (fp32 [1]) = fp32(sum |d| / (m C)), the sum in fp64
+ *   with per-block partials merged in a fixed order (NaN if any d is NaN, inf if any is infinite).
+ * osb_l1_head_bwd: with g (fp32 [1], the upstream gradient of loss) read on the device (no host sync), s = fp32(g * fp32(1 /
+ *   fp32(m C))) and dloss/df = s sgn(d) from the signs; dx_split [n, cin] = s (sgn_r w^T) at rows[r] and exactly 0 on every
+ *   other row; dw (fp32 [cin, C], overwritten) = s (X^T Sgn), per-split fp32 partials merged in fp64 in a fixed order.  Two
+ *   calls give identical bits. */
+size_t osb_l1_head_workspace_bytes(int64_t m, int32_t cin, int32_t C);
+int osb_l1_head_fwd(const void *x_split, int64_t n, int32_t cin, const float *w, int32_t C, const int32_t *rows, int64_t m,
+                    const void *target, uint32_t *signs, float *loss, void *ws, size_t ws_bytes, void *stream);
+int osb_l1_head_bwd(const void *x_split, int64_t n, int32_t cin, const float *w, int32_t C, const int32_t *rows, int64_t m,
+                    const uint32_t *signs, const float *g, void *dx_split, float *dw, void *ws, size_t ws_bytes, void *stream);
+
 /* fp32 [n,c] <-> split rows. */
 int osb_f32_to_split(const float *in, int64_t n, int32_t c, void *out_split, void *stream);
 int osb_split_to_f32(const void *in_split, int64_t n, int32_t c, float *out, void *stream);

@@ -61,6 +61,9 @@ SIGNATURES = {
     'osb_cos_head_workspace_bytes': (SZ, [I64, I32, I32]),
     'osb_cos_head_fwd': (c_int, [P, I64, I32, P, I32, P, I64, P, P, P, P, SZ, P]),
     'osb_cos_head_bwd': (c_int, [P, I64, I32, P, I32, P, I64, P, P, P, P, P, P, SZ, P]),
+    'osb_l1_head_workspace_bytes': (SZ, [I64, I32, I32]),
+    'osb_l1_head_fwd': (c_int, [P, I64, I32, P, I32, P, I64, P, P, P, P, SZ, P]),
+    'osb_l1_head_bwd': (c_int, [P, I64, I32, P, I32, P, I64, P, P, P, P, P, SZ, P]),
     'osb_f32_to_split': (c_int, [P, I64, I32, P, P]),
     'osb_split_to_f32': (c_int, [P, I64, I32, P, P]),
     'osb_gather_rows_f32': (c_int, [P, P, I64, I32, P, P]),

@@ -42,6 +42,7 @@
 //                   k_cos_head_dw_out adds H W (H the X part) in fp64.
 // Every assignment of rows to blocks and every merge order is a function of (m, cin, C) only: two calls give identical bits.
 #include "common.cuh"
+#include "head_tile.cuh"
 #include <algorithm>
 #include <math.h>
 
@@ -97,29 +98,11 @@ static size_t cos_ws_layout(int64_t m, int cin, int c, void *base, CosWs *out) {
 // torch's clamp_min: NaN stays NaN
 __device__ inline double cos_clamp(double v) { return v < COS_EPS ? COS_EPS : v; }
 
-// channels 8 q .. 8 q + 7 of a 128-byte split line
-__device__ inline void cos_load8(const uint8_t *line, int q, float v[8]) {
-  union { uint4 u; __nv_bfloat16 b[8]; } hi, lo;
-  hi.u = __ldg(reinterpret_cast<const uint4 *>(line + 16 * q));
-  lo.u = __ldg(reinterpret_cast<const uint4 *>(line + 64 + 16 * q));
-#pragma unroll
-  for (int j = 0; j < 8; ++j) v[j] = join_bf16(hi.b[j], lo.b[j]);
-}
-
 __device__ inline void cos_load_t8(const __half *t, float v[8]) {
   union { uint4 u; __half h[8]; } x;
   x.u = __ldg(reinterpret_cast<const uint4 *>(t));
 #pragma unroll
   for (int j = 0; j < 8; ++j) v[j] = __half2float(x.h[j]);
-}
-
-// acc[e][f] += a[e] b[f]
-__device__ inline void cos_fma44(float acc[4][4], const float4 a, const float4 b) {
-  const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-  for (int e = 0; e < 4; ++e)
-#pragma unroll
-    for (int f = 0; f < 4; ++f) acc[e][f] = fmaf(av[e], bv[f], acc[e][f]);
 }
 
 // forward: per 64-row tile, f = x W column tile by column tile, row sums in fp64: state[r] = (|f|^2, f.t, |t|^2)
@@ -138,7 +121,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_fwd(const uint8_t *__r
       const int r = u / units, q = u - r * units;
       float v[8];
       if (i0 + r < m) {
-        cos_load8(x + (int64_t)__ldg(rows + i0 + r) * row_bytes + 128 * (q >> 2), q & 3, v);
+        head_load8(x + (int64_t)__ldg(rows + i0 + r) * row_bytes + 128 * (q >> 2), q & 3, v);
       } else {
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = 0.f;
@@ -165,7 +148,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_fwd(const uint8_t *__r
         __syncthreads();
 #pragma unroll 8
         for (int kk = 0; kk < 32; ++kk)
-          cos_fma44(acc, *reinterpret_cast<const float4 *>(xs + (k0 + kk) * COS_FWD_LD + 4 * ty),
+          head_fma44(acc, *reinterpret_cast<const float4 *>(xs + (k0 + kk) * COS_FWD_LD + 4 * ty),
                     *reinterpret_cast<const float4 *>(ws + kk * 64 + 4 * tx));
       }
 #pragma unroll
@@ -317,7 +300,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_dx(const uint8_t *__re
     __syncthreads();
 #pragma unroll 8
     for (int d = 0; d < 32; ++d)
-      cos_fma44(p, *reinterpret_cast<const float4 *>(&as[d][4 * ty]), *reinterpret_cast<const float4 *>(&bs[d][4 * tx]));
+      head_fma44(p, *reinterpret_cast<const float4 *>(&as[d][4 * ty]), *reinterpret_cast<const float4 *>(&bs[d][4 * tx]));
   }
   for (int k0 = 0; k0 < cin; k0 += 32) {                     // Q = X G
     __syncthreads();
@@ -325,7 +308,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_dx(const uint8_t *__re
       const int r = u >> 2, qq = u & 3;
       float v[8];
       if (i0 + r < m) {
-        cos_load8(x + (int64_t)__ldg(rows + i0 + r) * row_bytes + 4 * k0, qq, v);
+        head_load8(x + (int64_t)__ldg(rows + i0 + r) * row_bytes + 4 * k0, qq, v);
       } else {
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = 0.f;
@@ -341,7 +324,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_dx(const uint8_t *__re
     __syncthreads();
 #pragma unroll 8
     for (int d = 0; d < 32; ++d)
-      cos_fma44(q, *reinterpret_cast<const float4 *>(&as[d][4 * ty]), *reinterpret_cast<const float4 *>(&bs[d][4 * tx]));
+      head_fma44(q, *reinterpret_cast<const float4 *>(&as[d][4 * ty]), *reinterpret_cast<const float4 *>(&bs[d][4 * tx]));
   }
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
@@ -384,7 +367,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_dw(const uint8_t *__re
       const int r = tid >> 2, qq = tid & 3;
       float v[8];
       if (r < nr) {
-        cos_load8(x + (int64_t)__ldg(rows + base + r) * row_bytes + 128 * kb, qq, v);
+        head_load8(x + (int64_t)__ldg(rows + base + r) * row_bytes + 128 * kb, qq, v);
       } else {
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = 0.f;
@@ -405,7 +388,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_dw(const uint8_t *__re
           for (int j = 0; j < 8; ++j) v[j] *= s.x;
         } else {
           const int ch = col - c;
-          cos_load8(x + (int64_t)__ldg(rows + i) * row_bytes + 128 * (ch >> 5), (ch & 31) >> 3, v);
+          head_load8(x + (int64_t)__ldg(rows + i) * row_bytes + 128 * (ch >> 5), (ch & 31) >> 3, v);
 #pragma unroll
           for (int j = 0; j < 8; ++j) v[j] *= s.y;
         }
@@ -418,7 +401,7 @@ __global__ void __launch_bounds__(COS_THREADS) k_cos_head_dw(const uint8_t *__re
     }
     __syncthreads();
     for (int r = 0; r < nr; ++r)
-      cos_fma44(acc, *reinterpret_cast<const float4 *>(&xa[r][4 * kq]), *reinterpret_cast<const float4 *>(&bs[r][4 * cg]));
+      head_fma44(acc, *reinterpret_cast<const float4 *>(&xa[r][4 * kq]), *reinterpret_cast<const float4 *>(&bs[r][4 * cg]));
   }
   const int col = col0 + 4 * cg;
   if (col < w2) {

@@ -115,14 +115,27 @@ def fused_cosine_step(engine, optimizer, coords, feats, feat_3d, mask, translate
     """``fused_distill_step`` with the cosine loss on the engine's device head: the same random translation, zero_grad,
     backward and optimiser step, with ``engine.forward_train_cosine`` in place of ``forward_train`` + ``distill_loss``, so
     the [M, C] output rows and their gradient are never materialised.  ``feat_3d`` is cast to fp16 on the engine's device
-    (the dtype run/distill.py's targets have).  The L1 loss stays on ``fused_distill_step``."""
-    refuse_local_engine(engine, 'fused_cosine_step')
+    (the dtype run/distill.py's targets have).  The L1 loss has its own device head: ``fused_l1_step``."""
+    return _fused_head_step(engine, optimizer, coords, feats, feat_3d, mask, translate, 'fused_cosine_step',
+                            engine.forward_train_cosine)
+
+
+def fused_l1_step(engine, optimizer, coords, feats, feat_3d, mask, translate=True):
+    """``fused_distill_step(..., loss_type='l1')`` on the engine's device L1 head: ``fused_cosine_step`` with
+    ``engine.forward_train_l1`` (the same translation draw, zero_grad, backward and optimiser step; bound ``optim.Adam`` /
+    ``optim.SGD``, ``torch.optim`` and ``process_group`` engines alike)."""
+    return _fused_head_step(engine, optimizer, coords, feats, feat_3d, mask, translate, 'fused_l1_step',
+                            engine.forward_train_l1)
+
+
+def _fused_head_step(engine, optimizer, coords, feats, feat_3d, mask, translate, what, forward):
+    refuse_local_engine(engine, what)
     if translate:
         coords = coords.clone()
         coords[:, 1:4] += (torch.rand(3) * 100).type_as(coords)
     dev = engine.device
-    loss = engine.forward_train_cosine(coords.to(dev, non_blocking=True), feats.to(dev, non_blocking=True),
-                                       feat_3d.to(dev, torch.float16), mask.to(dev))
+    loss = forward(coords.to(dev, non_blocking=True), feats.to(dev, non_blocking=True), feat_3d.to(dev, torch.float16),
+                   mask.to(dev))
     optimizer.zero_grad()
     loss.backward()
     optimizer.step()

@@ -109,7 +109,7 @@ class FusedMinkUNet:
         self._bs_ws = None
         self._gen = 0                             # bumped by every forward: a training graph whose activations were overwritten
         self._garena = []                         # training: grow-only chunks of gradient rows (engine_train.py)
-        self._ce_ws = None                        # workspace of the cross-entropy and cosine heads (engine_train.py, forward_eval_ce)
+        self._ce_ws = None                        # workspace of the CE, cosine and L1 heads (engine_train.py, forward_eval_ce)
         self._build()
         self.out_channels = self.final.cout
         self.last_cm = None
@@ -578,6 +578,14 @@ class FusedMinkUNet:
         [M, C] rows and their gradient are never materialised (openscene_b200/engine_train.py, csrc/cos_head.cu)."""
         from . import engine_train
         return self._dp_forward(engine_train.forward_train_cosine, self, coords, feats, feat_3d, rows)
+
+    def forward_train_l1(self, coords, feats, feat_3d, rows):
+        """Distillation step with run/distill.py's L1 loss on a batch_stats engine: returns the 0-dim fp32 loss
+        ``distill_loss(forward_train(coords, feats, rows), feat_3d, 'l1')`` with a grad_fn; arguments and supported heads as
+        in forward_train_cosine.  The [M, C] rows and their gradient are never materialised; the backward reads the 2-bit
+        signs of f - t the forward kept (openscene_b200/engine_train.py, csrc/l1_head.cu)."""
+        from . import engine_train
+        return self._dp_forward(engine_train.forward_train_l1, self, coords, feats, feat_3d, rows)
 
     @torch.no_grad()
     def forward_eval_ce(self, coords, feats, labels, inds_reverse, loss, areas, bad, ignore_index=255, pred=None):

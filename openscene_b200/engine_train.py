@@ -22,6 +22,8 @@ residual never alias), so two identical steps give bit-identical gradients.
 ``osb_ce_head_bwd``, which writes the head's weight gradient and the trunk output's gradient, and continues as above.
 ``forward_train_cosine`` (distillation with run/distill.py's cosine loss) does the same with ``osb_cos_head_fwd`` (head product
 and cosine loss on the selected rows) and ``osb_cos_head_bwd``: the C-wide rows and their gradient never exist.
+``forward_train_l1`` (the L1 loss) does the same with ``osb_l1_head_fwd`` (head product, L1 loss and the packed signs of
+f - t) and ``osb_l1_head_bwd`` (the gradients from the signs alone).
 
 With a process group (``FusedMinkUNet(model, batch_stats=True, process_group=pg)``) the backward all-reduces the gradients as
 DistributedDataParallel does: the flat gradient buffer is cut at parameter boundaries into buckets, from the end of the
@@ -130,7 +132,7 @@ def forward_train_ce(eng, coords, feats, labels, ignore_index=-100):
 
 
 def _ce_workspace(eng, n, cin, c, query='osb_ce_head_workspace_bytes'):
-    """the engine's head workspace (shared by the cross-entropy and cosine heads), grown to the query's size"""
+    """the engine's head workspace (shared by the cross-entropy, cosine and L1 heads), grown to the query's size"""
     need = getattr(C.lib(), query)(n, cin, c)
     if eng._ce_ws is None or eng._ce_ws.numel() < need:
         eng._ce_ws = None
@@ -201,27 +203,32 @@ def forward_train_cosine(eng, coords, feats, feat_3d, rows):
     The trunk runs as in forward_train; the final 1x1x1 layer and the loss are one launch (osb_cos_head_fwd) and their
     backward another (osb_cos_head_bwd): the [M, C] rows and their gradient never exist.  feat_3d: fp16 [M, C] on the
     engine's device, in the order of ``rows`` (bool mask or int64 caller-row index, as in forward_train)."""
+    _refuse_distill_head(eng, feats, feat_3d, rows, 'forward_train_cosine')
+    params = list(eng._net.parameters())
+    return _CosFunction.apply(eng, coords, feats, rows, feat_3d.contiguous(), *params)
+
+
+def _refuse_distill_head(eng, feats, feat_3d, rows, what):
+    """everything the device distillation heads refuse, before anything is launched; re-packs a stale engine"""
     _refuse(eng, feats)
     C.require_cuda(feats, 'features')
     if eng._sig != eng._signature():
         eng.refresh()
     fin = eng.final
     if fin.cout not in COS_WIDTHS or fin.cin not in CE_CIN or fin.K != 1:
-        raise NotImplementedError(f"forward_train_cosine: a 1x1x1 head of {fin.cin} -> {fin.cout} channels (supported: input "
+        raise NotImplementedError(f"{what}: a 1x1x1 head of {fin.cin} -> {fin.cout} channels (supported: input "
                                   f"width a multiple of 32 up to 384, output width 512 or 768); train it with forward_train "
                                   f"and distill_loss")
     if not isinstance(feat_3d, torch.Tensor) or feat_3d.dtype != torch.float16:
-        raise TypeError(f"forward_train_cosine: feat_3d must be an fp16 tensor (got {getattr(feat_3d, 'dtype', type(feat_3d))})")
+        raise TypeError(f"{what}: feat_3d must be an fp16 tensor (got {getattr(feat_3d, 'dtype', type(feat_3d))})")
     if feat_3d.dim() != 2 or feat_3d.shape[1] != fin.cout:
-        raise ValueError(f"forward_train_cosine: feat_3d of shape {tuple(feat_3d.shape)} for a head of {fin.cout} channels "
+        raise ValueError(f"{what}: feat_3d of shape {tuple(feat_3d.shape)} for a head of {fin.cout} channels "
                          f"(expected [M, {fin.cout}])")
     if feat_3d.device != eng.device:
-        raise ValueError(f"forward_train_cosine: feat_3d is on {feat_3d.device}, the engine on {eng.device}")
+        raise ValueError(f"{what}: feat_3d is on {feat_3d.device}, the engine on {eng.device}")
     if rows is None:
-        raise ValueError("forward_train_cosine: rows (the supervised rows) is required")
+        raise ValueError(f"{what}: rows (the supervised rows) is required")
     _ensure_bwd_packs(eng)
-    params = list(eng._net.parameters())
-    return _CosFunction.apply(eng, coords, feats, rows, feat_3d.contiguous(), *params)
 
 
 def _cos_forward(eng, cur, n0, sel, target, tape):
@@ -258,6 +265,65 @@ class _CosFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, eng, coords, feats, rows, target, *params):
         graph = _run_forward(eng, coords, feats, rows, cos=target)
+        loss = graph.out
+        graph.out = None
+        ctx.eng, ctx.graph = eng, graph
+        ctx.save_for_backward(*params)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        params = ctx.saved_tensors
+        grads = _run_backward(ctx.eng, ctx.graph, g, params)
+        ctx.graph = None
+        return (None, None, None, None, None) + tuple(grads)
+
+
+def forward_train_l1(eng, coords, feats, feat_3d, rows):
+    """0-dim fp32 loss with a grad_fn: ``distill_loss(forward_train(coords, feats, rows), feat_3d, 'l1')``, the mean of
+    |f - t| over the [M, C] elements.  The trunk runs as in forward_train; the final 1x1x1 layer and the loss are one launch
+    sequence (osb_l1_head_fwd, which keeps the 2-bit sign of every f - t) and their backward another (osb_l1_head_bwd, from
+    the signs alone): the [M, C] rows and their gradient never exist.  feat_3d and rows as in forward_train_cosine."""
+    _refuse_distill_head(eng, feats, feat_3d, rows, 'forward_train_l1')
+    params = list(eng._net.parameters())
+    return _L1Function.apply(eng, coords, feats, rows, feat_3d.contiguous(), *params)
+
+
+def _l1_forward(eng, cur, n0, sel, target, tape):
+    """osb_l1_head_fwd on the trunk's last activation; records the signs the backward reads"""
+    fin, dev = eng.final, eng.device
+    m = sel.shape[0]
+    signs = torch.empty((m, fin.cout // 16), dtype=torch.int32, device=dev)      # uint32 words (torch has no uint32 kernels)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    ws_a, ws_b = _ce_workspace(eng, m, cur[1], fin.cout, 'osb_l1_head_workspace_bytes')
+    rc = C.lib().osb_l1_head_fwd(cur[0], n0, cur[1], fin.w3.data_ptr(), fin.cout, sel.data_ptr(), m, target.data_ptr(),
+                                 signs.data_ptr(), loss.data_ptr(), ws_a, ws_b, eng._stream)
+    if rc:
+        C.check(rc, 'osb_l1_head_fwd')
+    tape.append(('l1_head', (_Node(fin, 0, 0, n0, [cur], 1, 0, 0), sel, signs)))
+    return loss
+
+
+def _l1_backward(eng, item, g, slot, galloc, grads, stream):
+    """osb_l1_head_bwd: dW into the final kernel's gradient slot, dx = the gradient of the trunk's last activation"""
+    nd, sel, signs = item
+    cv = nd.cv
+    (src, c, n0), = nd.srcs
+    m = sel.shape[0]
+    dx = galloc(n0 * 4 * c)
+    ws_a, ws_b = _ce_workspace(eng, m, c, cv.cout, 'osb_l1_head_workspace_bytes')
+    rc = C.lib().osb_l1_head_bwd(src, n0, c, cv.w3.data_ptr(), cv.cout, sel.data_ptr(), m, signs.data_ptr(), g.data_ptr(), dx,
+                                 slot(cv.mod.kernel).data_ptr(), ws_a, ws_b, stream)
+    if rc:
+        C.check(rc, 'osb_l1_head_bwd')
+    grads[src] = dx
+
+
+class _L1Function(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, eng, coords, feats, rows, target, *params):
+        graph = _run_forward(eng, coords, feats, rows, l1=target)
         loss = graph.out
         graph.out = None
         ctx.eng, ctx.graph = eng, graph
@@ -336,7 +402,7 @@ class _TrainFunction(torch.autograd.Function):
         return (None, None, None, None) + tuple(grads)
 
 
-def _run_forward(eng, coords, feats, rows, ce=None, cos=None):
+def _run_forward(eng, coords, feats, rows, ce=None, cos=None, l1=None):
     dev = eng.device
     st = eng.stem
     with torch.cuda.device(dev):
@@ -351,8 +417,9 @@ def _run_forward(eng, coords, feats, rows, ce=None, cos=None):
                 raise ValueError(f"Expected more than 1 value per channel when training, got input size [{n[l]}, {c}] "
                                  f"(level {l}, tensor stride {ts[l]})")
         sel = _select(cm, rows, n[0], dev) if ce is None else None
-        if cos is not None and cos.shape[0] != sel.shape[0]:
-            raise ValueError(f"forward_train_cosine: feat_3d has {cos.shape[0]} rows for {sel.shape[0]} selected rows")
+        for what, tgt in (('forward_train_cosine', cos), ('forward_train_l1', l1)):
+            if tgt is not None and tgt.shape[0] != sel.shape[0]:
+                raise ValueError(f"{what}: feat_3d has {tgt.shape[0]} rows for {sel.shape[0]} selected rows")
         eng._gen += 1                                    # from here on the arena is overwritten
         eng.last_cm = cm
         m3 = [cm.kernel_map(t, t, 3) for t in ts]
@@ -363,7 +430,7 @@ def _run_forward(eng, coords, feats, rows, ce=None, cos=None):
         m, sel_t = n[0], None
         if ce is None:
             m = sel.shape[0]
-        if ce is None and cos is None:
+        if ce is None and cos is None and l1 is None:
             sel_t = torch.empty(n[0], dtype=torch.int32, device=dev)
             C.call('osb_kernel_map_transpose', C.ptr(sel), m, 1, C.ptr(sel_t), n[0], C.stream_ptr())
         k5 = cm.kernel_map(1, 1, st.ks)
@@ -477,6 +544,8 @@ def _run_forward(eng, coords, feats, rows, ce=None, cos=None):
         fin = eng.final
         if cos is not None:
             out = _cos_forward(eng, cur, n[0], sel, cos, tape)
+        elif l1 is not None:
+            out = _l1_forward(eng, cur, n[0], sel, l1, tape)
         elif ce is None:
             out = torch.empty((m, fin.cout), dtype=torch.float32, device=dev)
             rc = eng._fn(cur[0], cur[1], n[0], 0, 0, 0, sel.data_ptr(), m, 1, fin.wpack_a, fin.cout, 0, 0, 0, 0, 0, out.data_ptr(),
@@ -504,7 +573,7 @@ def plan_buckets(tape, params):
     index = {id(p): i for i, p in enumerate(params)}
     last = [None] * len(params)
     for t, (kind, item) in enumerate(reversed(tape)):
-        nodes = item if kind == 'block' else (item[0] if kind in ('ce_head', 'cos_head') else item,)
+        nodes = item if kind == 'block' else (item[0] if kind in ('ce_head', 'cos_head', 'l1_head') else item,)
         for nd in nodes:
             if nd is not None:
                 bn = nd.cv.bn
@@ -656,6 +725,8 @@ def _run_backward(eng, gr, g, params):
                 _ce_backward(eng, item, g, slot, galloc, grads, stream)
             elif kind == 'cos_head':
                 _cos_backward(eng, item, g, slot, galloc, grads, stream)
+            elif kind == 'l1_head':
+                _l1_backward(eng, item, g, slot, galloc, grads, stream)
             elif kind == 'block':
                 n1, nd_, n2 = item
                 g2 = grads[n2.y]

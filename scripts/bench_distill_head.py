@@ -1,9 +1,11 @@
 #!/usr/bin/env python
 """The distillation step's head on the fused engine: ``distill.fused_distill_step`` (tensor-core head launch, torch's cosine
 loss chain on the fp32 [M, 768] rows, the split conversion of their gradient, head wgrad and dgrad) against
-``distill.fused_cosine_step`` (osb_cos_head_fwd / osb_cos_head_bwd), both with ``optim.Adam`` bound to the engine.
+``distill.fused_cosine_step`` (osb_cos_head_fwd / osb_cos_head_bwd), both with ``optim.Adam`` bound to the engine; with
+--loss l1, ``fused_distill_step(loss_type='l1')`` (torch's L1 chain) against ``distill.fused_l1_step`` (osb_l1_head_fwd /
+osb_l1_head_bwd).
 
-    python scripts/bench_distill_head.py [--steps K] [--warmup W] [--out DIR]
+    python scripts/bench_distill_head.py [--loss cosine|l1] [--steps K] [--warmup W] [--out DIR]
 
 Workloads: one synth.scene('config2_200k') with 20,000 supervised rows on MinkUNet18A and MinkUNet34C (the config3_distill
 shape), and 8 synth.scene('config1_50k') scenes with 20,000 rows each (160,000 rows) on MinkUNet18A (the one-GPU ScanNet /
@@ -18,9 +20,10 @@ work, L2 flushed before each, alternating.  Kernel counts per step and per head 
 Reported per workload: ms per step and per head (min / median / max), kernels per step and per head, peak memory per step, the
 loss difference and the largest per-parameter gradient difference (relative to that parameter's largest gradient) after one
 step from the same state; and the device name, power limit and SM clocks sampled during the run.  The JSON line is printed
-and, with --out, written to DIR/bench_distill_head.json."""
+and, with --out, written to DIR/bench_distill_head.json (--loss l1: DIR/bench_distill_head_l1.json)."""
 import argparse
 import copy
+import functools
 import gc
 import json
 import os
@@ -75,6 +78,7 @@ def main():
     ap.add_argument('--rows', type=int, default=20000)
     ap.add_argument('--workloads', default='0,1,2')
     ap.add_argument('--out', default=None)
+    ap.add_argument('--loss', choices=('cosine', 'l1'), default='cosine')
     args = ap.parse_args()
 
     from bench import ClockSampler
@@ -87,7 +91,8 @@ def main():
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     power_w, power_how = power_limit_w(0)
     sampler = ClockSampler(0, dev)
-    result = {'metric': 'ms per distillation step (translate, forward, cosine loss, backward, bound Adam) and per head',
+    new = args.loss                                                  # the arm and head names: cosine_step / l1_step, ...
+    result = {'metric': f'ms per distillation step (translate, forward, {new} loss, backward, bound Adam) and per head',
               'device': torch.cuda.get_device_name(dev), 'power_limit_w': power_w, 'power_limit_source': power_how,
               'steps': args.steps, 'warmup': args.warmup, 'rows_per_scene': args.rows,
               'method': 'weights, buffers and Adam state restored in place, re-packed, L2 flushed before every step and every '
@@ -99,7 +104,9 @@ def main():
         coords, feats, mask, tgt = _data(scene, k, args.rows, dev)
         base = synth.build_model(arch, 768, seed=0).train().to(dev)
         arms = {}
-        for name, step in (('distill_step', distill.fused_distill_step), ('cosine_step', distill.fused_cosine_step)):
+        new_step = distill.fused_cosine_step if new == 'cosine' else distill.fused_l1_step
+        for name, step in (('distill_step', functools.partial(distill.fused_distill_step, loss_type=new)),
+                           (f'{new}_step', new_step)):
             m = copy.deepcopy(base)
             eng = engine.FusedMinkUNet(m, batch_stats=True)
             o = optim.Adam(m.parameters(), lr=1e-3)
@@ -141,7 +148,7 @@ def main():
             losses[name] = float(step(eng, keep, coords, feats, tgt, mask))
             grads[name] = [p.grad.clone() for p in m.parameters()]
         gdiff = max(float((a - b).abs().max() / (b.abs().max() + 1e-30))
-                    for a, b in zip(grads['cosine_step'], grads['distill_step']))
+                    for a, b in zip(grads[f'{new}_step'], grads['distill_step']))
         del grads
         evs, peak = {n: [] for n in arms}, {}
         gc.collect()
@@ -165,12 +172,12 @@ def main():
         finally:
             gc.enable()
         rec = {'rows': int(mask.sum()), 'voxels': int(coords.shape[0]), 'arch': arch,
-               'loss_distill_step': losses['distill_step'], 'loss_cosine_step': losses['cosine_step'],
-               'loss_rel_diff': abs(losses['cosine_step'] - losses['distill_step']) / abs(losses['distill_step']),
+               'loss_distill_step': losses['distill_step'], f'loss_{new}_step': losses[f'{new}_step'],
+               'loss_rel_diff': abs(losses[f'{new}_step'] - losses['distill_step']) / abs(losses['distill_step']),
                'max_param_grad_diff_rel_to_max': gdiff, 'peak_mem_gib': peak}
         for name, pairs in evs.items():
             rec[name] = _stats([a.elapsed_time(b) for a, b in pairs])
-        rec['step_speedup_median'] = rec['distill_step']['ms_median'] / rec['cosine_step']['ms_median']
+        rec['step_speedup_median'] = rec['distill_step']['ms_median'] / rec[f'{new}_step']['ms_median']
         rec['kernels_per_step'] = {}
         for name in arms:
             restore(name)
@@ -194,8 +201,10 @@ def main():
         gsplit = torch.empty((mm, 4 * cc), dtype=torch.uint8, device=dev)
         dw = torch.empty((cin, cc), device=dev)
         wg_ws = torch.empty(max(lib.osb_conv_wgrad_tc_workspace_bytes(mm, 1, cin, cc), 256), dtype=torch.uint8, device=dev)
-        cos_ws = torch.empty(lib.osb_cos_head_workspace_bytes(mm, cin, cc), dtype=torch.uint8, device=dev)
+        cos_ws = torch.empty(getattr(lib, f'osb_{"cos" if new == "cosine" else "l1"}_head_workspace_bytes')(mm, cin, cc),
+                             dtype=torch.uint8, device=dev)
         state = torch.empty((mm, 3), dtype=torch.float64, device=dev)
+        signs = torch.empty((mm, cc // 16), dtype=torch.int32, device=dev)
         loss = torch.empty((), device=dev)
         one = torch.ones((), device=dev)
 
@@ -204,7 +213,7 @@ def main():
             C.check(eng._fn(src, cin, n0, 0, 0, 0, nd.nbr_f, mm, 1, fin.wpack_a, cc, 0, 0, 0, 0, 0, f.data_ptr(), 0, eng._ws_a,
                             eng._ws_bytes, eng._flags, stream), 'osb_conv_fwd_tc')
             f.requires_grad_()
-            distill.distill_loss(f, tgt).backward()
+            distill.distill_loss(f, tgt, new).backward()
             C.call('osb_f32_to_split', C.ptr(f.grad), mm, cc, C.ptr(gsplit), C.stream_ptr())
             C.check(lib.osb_conv_wgrad_tc(src, cin, n0, nd.nbr_f, mm, 1, gsplit.data_ptr(), cc, dw.data_ptr(), wg_ws.data_ptr(),
                                           wg_ws.numel(), stream), 'osb_conv_wgrad_tc')
@@ -219,7 +228,14 @@ def main():
                                          state.data_ptr(), one.data_ptr(), dx.data_ptr(), dw.data_ptr(), cos_ws.data_ptr(),
                                          cos_ws.numel(), stream), 'osb_cos_head_bwd')
 
-        heads = {'old_head': old_head, 'cosine_head': new_head}
+        def l1_head():
+            C.check(lib.osb_l1_head_fwd(src, n0, cin, fin.w3.data_ptr(), cc, sel.data_ptr(), mm, tgt.data_ptr(), signs.data_ptr(),
+                                        loss.data_ptr(), cos_ws.data_ptr(), cos_ws.numel(), stream), 'osb_l1_head_fwd')
+            C.check(lib.osb_l1_head_bwd(src, n0, cin, fin.w3.data_ptr(), cc, sel.data_ptr(), mm, signs.data_ptr(), one.data_ptr(),
+                                        dx.data_ptr(), dw.data_ptr(), cos_ws.data_ptr(), cos_ws.numel(), stream),
+                    'osb_l1_head_bwd')
+
+        heads = {'old_head': old_head, f'{new}_head': new_head if new == 'cosine' else l1_head}
         for fn in heads.values():
             for _ in range(3):
                 fn()
@@ -239,10 +255,10 @@ def main():
         torch.cuda.synchronize()
         for name, pairs in hev.items():
             rec[name] = _stats([a.elapsed_time(b) for a, b in pairs])
-        rec['head_speedup_median'] = rec['old_head']['ms_median'] / rec['cosine_head']['ms_median']
+        rec['head_speedup_median'] = rec['old_head']['ms_median'] / rec[f'{new}_head']['ms_median']
         rec['head_extra_mem_gib'] = hpeak
         rec['kernels_per_head'] = {name: _kernels(fn) for name, fn in heads.items()}
-        rec['cosine_head_share_of_step'] = rec['cosine_head']['ms_median'] / rec['cosine_step']['ms_median']
+        rec[f'{new}_head_share_of_step'] = rec[f'{new}_head']['ms_median'] / rec[f'{new}_step']['ms_median']
         del out, gr, nd
         result['workloads'][label] = rec
         print(label, json.dumps(rec), flush=True)
@@ -253,7 +269,8 @@ def main():
     print(line)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, 'bench_distill_head.json'), 'w') as f:
+        name = 'bench_distill_head.json' if new == 'cosine' else 'bench_distill_head_l1.json'
+        with open(os.path.join(args.out, name), 'w') as f:
             f.write(line + '\n')
 
 
