@@ -431,6 +431,29 @@ int osb_match_ce(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c
                  int32_t classes, void *scores_f16, int64_t *pred, void *loss_f16, uint64_t *areas, int32_t *bad_labels,
                  void *ws, size_t ws_bytes, void *stream);
 
+/* Streaming top-k for vocabularies of any size: the product of osb_match_scores (same arguments, same fp16 scores s, the
+ * same bits for every column) over ceil(K / 96) passes, keeping per point p only the topk best columns, best first:
+ *   order    NaN above every number (NaNs by ascending column); numbers by descending value, -0 == +0, equal values by
+ *            ascending column.  topk = 1 is osb_match_vote's / osb_match_ce's argmax; on rows without NaN it is
+ *            osb_match_scores' label, on rows with a NaN it is not (osb_match_scores skips NaN).
+ *   label    int64 [n_pts, topk] (required), scores_f16 fp16 [n_pts, topk] (may be NULL): the columns and their scores
+ *   smax     fp32 [n_pts] (may be NULL): the largest non-NaN score at its lowest column, -inf when there is none, as
+ *            osb_match_scores reports it
+ * Nothing of size [n_pts, K] is written.  1 <= K <= OSB_MATCH_TOPK_MAX_TEXT, 1 <= topk <= min(8, K).  Tensor-core route
+ * only: OSB_MATCH_SIMT does not apply.  Two calls on the same inputs give the same bits. */
+#define OSB_MATCH_TOPK_MAX_TEXT 1048576
+int osb_match_topk(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c, const int64_t *inds_reverse,
+                   int64_t n_pts, const void *text_f16, int32_t k_text, int32_t normalize, int32_t topk, void *scores_f16,
+                   int64_t *label, float *smax, void *stream);
+/* The ensemble's final product as a streaming top-k (osb_match_ensemble with the order above):
+ *   fe = sel_a[p] < sel_b[p] ? feat2d_f16[v] : fp16(feat3d[v]);  label / scores_f16 = top-k of fe @ text^T
+ *   feat_out_f16 (may be NULL) receives fe.  sel_a / sel_b are the smax of two osb_match_topk calls with normalize = 1
+ *   (the 3-D and the 2-D features). */
+int osb_match_ensemble_topk(const float *feat3d, const void *feat2d_f16, int64_t n_vox, int32_t c,
+                            const int64_t *inds_reverse, int64_t n_pts, const float *sel_a, const float *sel_b,
+                            const void *text_f16, int32_t k_text, int32_t topk, void *scores_f16, int64_t *label,
+                            void *feat_out_f16, void *stream);
+
 /* Optional folded head (engine.forward_scores): rows z = [x L | x U] (fp32, row pitch ld floats) from one 1x1x1
  * convolution with the weights [L | U], W W^T = L L^T, U = W T^T  ->  score_k = fp16((x.U_k) / (|x L| + 1e-5)),
  * label = first argmax.  Same cosine scores as run/evaluate.py:305-310 without materialising the 768-d features. */

@@ -9,7 +9,8 @@
 // column holding the largest non-NaN score, and 0 when no score is above -inf (a row of NaN and -inf only); smax is that
 // largest non-NaN score, -inf when there is none.  Labels always lie in [0, K).  torch's CUDA `max(1)[1]`, which the
 // reference takes, returns a NaN's index instead; the repeat vote and the validation cross-entropy (k_match_tc_ce) follow
-// torch's CPU rule (vote.cuh).
+// torch's CPU rule (vote.cuh).  So does the streaming top-k (k_match_tc_topk): NaN first, and its label 0 is vote.cuh's
+// argmax; its smax is the rule above.
 #include "common.cuh"
 #include <algorithm>
 #include <stdlib.h>
@@ -147,6 +148,9 @@ int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, 
 int match_tc_ce_run(const void *feat, int feat_is_f16, int c, const int64_t *inds_reverse, int64_t n_pts, const void *text_f16,
                     int k_text, const void *label, int label_is_i64, int ignore, int classes, void *scores_f16, int64_t *pred,
                     void *loss_f16, uint64_t *areas, int32_t *bad, void *ws, cudaStream_t stream);
+int match_tc_topk_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
+                      const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize, int topk,
+                      void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, cudaStream_t stream);
 // CUDA-core repeat vote (vote.cu)
 int vote_accumulate_run(const void *src, int src_is_f16, const int64_t *inds_reverse, int64_t n_pts, int k, void *store,
                         int64_t *label_cur, int64_t *label_acc, cudaStream_t stream);
@@ -288,6 +292,40 @@ int osb_match_ce(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c
             "osb_match_ce: 8-byte aligned workspace of %zu bytes required (got %zu)", need, ws_bytes);
   return match_tc_ce_run(feat, feat_is_f16, c, inds_reverse, n_pts, text_f16, k_text, label, label_is_i64, ignore_index,
                          classes, scores_f16, pred, loss_f16, areas, bad_labels, ws, stream);
+}
+
+// Streaming top-k over any number of 96-row passes; tensor-core route only.
+static int check_topk_args(const char *fn, int32_t c, int32_t k_text, int32_t topk, int64_t n_vox, int64_t n_pts,
+                           const void *text_f16, const int64_t *label) {
+  OSB_CHECK(c == 512 || c == 768, "%s: feature width %d unsupported (OpenScene uses 512 / 768)", fn, c);
+  OSB_CHECK(k_text >= 1 && k_text <= OSB_MATCH_TOPK_MAX_TEXT, "%s: K_text=%d outside 1..%d", fn, k_text,
+            OSB_MATCH_TOPK_MAX_TEXT);
+  OSB_CHECK(topk >= 1 && topk <= std::min(8, k_text), "%s: topk=%d outside 1..min(8, K_text=%d)", fn, topk, k_text);
+  OSB_CHECK(n_vox > 0 && n_pts >= 0, "%s: bad shape (n_vox=%lld, n_pts=%lld)", fn, (long long)n_vox, (long long)n_pts);
+  OSB_CHECK(text_f16 != nullptr, "%s: NULL text", fn);
+  OSB_CHECK(label != nullptr, "%s: NULL label", fn);
+  return 0;
+}
+
+int osb_match_topk(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t c, const int64_t *inds_reverse,
+                   int64_t n_pts, const void *text_f16, int32_t k_text, int32_t normalize, int32_t topk, void *scores_f16,
+                   int64_t *label, float *smax, void *stream_) {
+  if (check_topk_args("osb_match_topk", c, k_text, topk, n_vox, n_pts, text_f16, label)) return 1;
+  OSB_CHECK(feat != nullptr, "osb_match_topk: NULL features");
+  if (n_pts == 0) return 0;
+  return match_tc_topk_run(feat, feat_is_f16, nullptr, nullptr, nullptr, c, inds_reverse, n_pts, text_f16, k_text, normalize,
+                           topk, scores_f16, label, smax, nullptr, (cudaStream_t)stream_);
+}
+
+int osb_match_ensemble_topk(const float *feat3d, const void *feat2d_f16, int64_t n_vox, int32_t c,
+                            const int64_t *inds_reverse, int64_t n_pts, const float *sel_a, const float *sel_b,
+                            const void *text_f16, int32_t k_text, int32_t topk, void *scores_f16, int64_t *label,
+                            void *feat_out_f16, void *stream_) {
+  if (check_topk_args("osb_match_ensemble_topk", c, k_text, topk, n_vox, n_pts, text_f16, label)) return 1;
+  OSB_CHECK(feat3d && feat2d_f16 && sel_a && sel_b, "osb_match_ensemble_topk: NULL features or row maxima");
+  if (n_pts == 0) return 0;
+  return match_tc_topk_run(feat3d, 0, feat2d_f16, sel_a, sel_b, c, inds_reverse, n_pts, text_f16, k_text, 0, topk, scores_f16,
+                           label, nullptr, feat_out_f16, (cudaStream_t)stream_);
 }
 
 }  // extern "C"

@@ -21,6 +21,10 @@
 // k_match_tc_ce is the same kernel with the validation tail of run/distill.py in the epilogue (MatchTcCe below): the
 // cross-entropy term, the argmax and the intersection / union / target counts of every row.  k_match_tc and
 // k_match_tc_vote compile to the same instructions as before it existed.
+//
+// k_match_tc_topk is the same kernel with a running per-point top-k (k <= 8) in the epilogue (MatchTcTopk below), so the
+// number of passes has no bound of its own: the result is [N_pts, k], never [N_pts, K].  The three kernels above compile
+// to the same instructions as before it existed.
 #include "metric.cuh"
 #include "tc_ptx.cuh"
 #include "vote.cuh"
@@ -71,7 +75,35 @@ struct MatchTcCe {
   void *loss;                        // fp16 [1]: fp16(sum / rows), written by k_match_ce_loss
 };
 
-enum { MT_PLAIN = 0, MT_VOTE = 1, MT_CE = 2 };
+// Streaming top-k (k_match_tc_topk): per point, the k best of all K fp16 scores, best first.  NaN ranks above every
+// number (NaNs by ascending column), numbers by descending value with -0 == +0, equal values by ascending column; k = 1
+// is vote.cuh's rule.  Each row keeps its list of k order keys (topk_key) in shared memory; a column is tested against
+// the upper half of the row's k-th key, read once per pass, and only the columns that pass are offered to the list, one
+// lane of the row's quad at a time.
+struct MatchTcTopk {
+  int k;                             // 1..8, at most K
+  __half *scores;                    // [n_pts, k] or NULL
+  int64_t *label;                    // [n_pts, k]
+};
+constexpr int MT_TOPK_MAX = 8;
+
+enum { MT_PLAIN = 0, MT_VOTE = 1, MT_CE = 2, MT_TOPK = 3 };
+
+// order key of score h at column k: larger is better.  Bits 48-63 map the score to an unsigned order (NaN highest, -0 as
+// +0), bits 16-47 hold ~k (the lower column wins a tie), bits 0-15 the score's own fp16 bits.  Every valid key is > 0.
+__device__ __forceinline__ uint64_t topk_key(__half h, int k) {
+  const uint32_t b = __half_as_ushort(h);
+  const uint32_t u = (b & 0x7fffu) > 0x7c00u ? 0xffffu : b == 0x8000u ? 0x8000u : (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
+  return ((uint64_t)u << 48) | ((uint64_t)(~(uint32_t)k) << 16) | b;
+}
+
+// insert key into the descending list L[0..n) unless it is below L[n-1] (keys are distinct: one per column)
+__device__ __forceinline__ void topk_insert(uint64_t *L, int n, uint64_t key) {
+  if (key < L[n - 1]) return;
+  int j = n - 1;
+  for (; j > 0 && L[j - 1] < key; --j) L[j] = L[j - 1];
+  L[j] = key;
+}
 
 // the label of point row pt as an int: y in [0, K), ignore, or (a label outside [0, K)) a negative value other than ignore
 __device__ __forceinline__ int ce_label(const MatchTcCe &ce, int64_t pt, int64_t n_pts, int k_text) {
@@ -84,8 +116,8 @@ __device__ __forceinline__ int ce_label(const MatchTcCe &ce, int64_t pt, int64_t
 
 template <int NP, int MODE>   // half2 pairs per lane: C = 64 * NP
 __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const MatchTcParams p, const MatchTcVote vo,
-                                              const MatchTcCe ce) {
-  constexpr bool VOTE = MODE == MT_VOTE, CE = MODE == MT_CE;
+                                              const MatchTcCe ce, const MatchTcTopk tk) {
+  constexpr bool VOTE = MODE == MT_VOTE, CE = MODE == MT_CE, TOPK = MODE == MT_TOPK;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int C = 64 * NP;
@@ -109,6 +141,8 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
   float *s_term = reinterpret_cast<float *>(sB + MT_BSTAGES * B_BYTES + 128);
   int *s_lab = reinterpret_cast<int *>(s_term + MT_M);
   uint32_t *s_hist = reinterpret_cast<uint32_t *>(s_lab + MT_M);
+  // TOPK: the block's 128 lists of MT_TOPK_MAX order keys
+  uint64_t *s_topk = reinterpret_cast<uint64_t *>(sB + MT_BSTAGES * B_BYTES + 128);
   if constexpr (CE)
     for (int b = tid; b < 3 * ce.classes; b += MT_THREADS) s_hist[b] = 0;
   __syncthreads();
@@ -223,6 +257,12 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
 #pragma unroll
       for (int h = 0; h < 2; ++h) { lm[h] = -INFINITY; ls[h] = 0.f; sy[h] = 0.f; vcur[h].init(); }
     }
+    if constexpr (TOPK) {   // empty lists: key 0 is below every valid key
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        for (int j = lane & 3; j < MT_TOPK_MAX; j += 4) s_topk[(r_lo + 8 * h) * MT_TOPK_MAX + j] = 0;
+      __syncwarp();
+    }
     mbar_wait(a_full, 0);
     int s = 0; uint32_t phase = 0;
     for (int pass = 0; pass < p.n_pass; ++pass) {
@@ -244,9 +284,9 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
         if ((tid & 127) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(b_empty + 8 * s) : "memory");
         if (++s == MT_BSTAGES) { s = 0; phase ^= 1; }
       }
-      // CE: this pass's fp16 scores of both rows as half2 pairs (the accumulators die here)
+      // CE, TOPK: this pass's fp16 scores of both rows as half2 pairs (the accumulators die here)
       __half2 hs[2][MT_NW / 8];
-      if constexpr (CE) {
+      if constexpr (CE || TOPK) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -259,6 +299,10 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
         int y = 0;
         float pm = -INFINITY;
         if constexpr (CE) y = ce_label(ce, pt, p.n_pts, p.k_text);
+        // TOPK: the row's k-th key, and the columns of this thread that beat it
+        uint64_t *row_topk = s_topk + (r_lo + 8 * h) * MT_TOPK_MAX;
+        uint32_t thr = 0, cand = 0;
+        if constexpr (TOPK) thr = (uint32_t)(row_topk[tk.k - 1] >> 32);
 #pragma unroll
         for (int i = 0; i < MT_NW / 8; ++i) {
           if constexpr (VOTE) {
@@ -307,6 +351,17 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
                 if (k == y) sy[h] = sc;
               }
             }
+          } else if constexpr (TOPK) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int k = pass * MT_NW + 8 * i + cq + e;
+              if (k < p.k_text) {
+                const __half hv = e ? __high2half(hs[h][i]) : __low2half(hs[h][i]);
+                const float sc = __half2float(hv);
+                if (sc > best[h]) { best[h] = sc; best_k[h] = k; }   // smax: the rule of the plain kernel
+                if ((uint32_t)(topk_key(hv, k) >> 32) >= thr) cand |= 1u << (2 * i + e);   // a superset of the survivors
+              }
+            }
           } else {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
@@ -331,6 +386,23 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
             if (k + 1 < p.k_text) sum += expf(f.y - mu);
           }
           lm[h] = mn; ls[h] = sum;
+        }
+        if constexpr (TOPK) {   // the survivors, one lane of each quad at a time (rare once the lists are full)
+          if (__any_sync(0xffffffffu, cand != 0)) {
+#pragma unroll 1
+            for (int q = 0; q < 4; ++q) {
+              if ((lane & 3) == q && cand != 0) {
+#pragma unroll
+                for (int i = 0; i < MT_NW / 8; ++i)
+#pragma unroll
+                  for (int e = 0; e < 2; ++e)
+                    if ((cand >> (2 * i + e)) & 1u)
+                      topk_insert(row_topk, tk.k,
+                                  topk_key(e ? __high2half(hs[h][i]) : __low2half(hs[h][i]), pass * MT_NW + 8 * i + cq + e));
+              }
+              __syncwarp();
+            }
+          }
         }
       }
     }
@@ -369,6 +441,26 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
           if (bad) atomicAdd(ce.bad, 1);
           else if (live) inter_union_add(vcur[h].k, y, ce.classes, ce.ignore, s_hist);
           if (live && p.label) p.label[pt] = vcur[h].k;
+        }
+      }
+    } else if constexpr (TOPK) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {   // smax as the plain kernel merges it
+          const float ob = __shfl_xor_sync(0xffffffffu, best[h], o);
+          const int ok = __shfl_xor_sync(0xffffffffu, best_k[h], o);
+          if (ob > best[h] || (ob == best[h] && ok < best_k[h])) { best[h] = ob; best_k[h] = ok; }
+        }
+        const int r = r_lo + 8 * h;
+        const int64_t pt = row0 + r;
+        if (pt < p.n_pts) {
+          for (int j = lane & 3; j < tk.k; j += 4) {
+            const uint64_t key = s_topk[r * MT_TOPK_MAX + j];
+            tk.label[pt * tk.k + j] = (int64_t)(~(uint32_t)(key >> 16));
+            if (tk.scores) tk.scores[pt * tk.k + j] = __ushort_as_half((unsigned short)(key & 0xffffu));
+          }
+          if ((lane & 3) == 0 && p.smax) p.smax[pt] = best[h];
         }
       }
     } else {
@@ -427,29 +519,44 @@ __global__ void __launch_bounds__(32) k_match_ce_loss(const double *__restrict__
 template <int NP>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 k_match_tc(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p) {
-  match_tc_body<NP, MT_PLAIN>(tmT, p, MatchTcVote{}, MatchTcCe{});
+  match_tc_body<NP, MT_PLAIN>(tmT, p, MatchTcVote{}, MatchTcCe{}, MatchTcTopk{});
 }
 
 template <int NP>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 k_match_tc_vote(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, const MatchTcVote vo) {
-  match_tc_body<NP, MT_VOTE>(tmT, p, vo, MatchTcCe{});
+  match_tc_body<NP, MT_VOTE>(tmT, p, vo, MatchTcCe{}, MatchTcTopk{});
 }
 
 template <int NP>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 k_match_tc_ce(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, const MatchTcCe ce) {
-  match_tc_body<NP, MT_CE>(tmT, p, MatchTcVote{}, ce);
+  match_tc_body<NP, MT_CE>(tmT, p, MatchTcVote{}, ce, MatchTcTopk{});
 }
 
-static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, const MatchTcCe *ce, const void *text_f16,
-                           cudaStream_t stream) {
+template <int NP>
+__global__ void __launch_bounds__(MT_THREADS, 1)
+k_match_tc_topk(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, const MatchTcTopk tk) {
+  match_tc_body<NP, MT_TOPK>(tmT, p, MatchTcVote{}, MatchTcCe{}, tk);
+}
+
+static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, const MatchTcCe *ce, const MatchTcTopk *tk,
+                           const void *text_f16, cudaStream_t stream) {
   CUtensorMap tmT;
   if (make_tmap_2b(&tmT, text_f16, (uint64_t)p.C, (uint64_t)p.k_text, MT_NW, 1)) return 1;
   const int NP = p.C / 64;
   const size_t smem = (size_t)NP * MT_M * 128 + MT_BSTAGES * MT_NW * 128 + 128 + 1024;
   const unsigned grid = (unsigned)ceil_div(p.n_pts, MT_M);
-  if (ce != nullptr) {
+  if (tk != nullptr) {
+    const size_t smem_tk = smem + (size_t)MT_M * MT_TOPK_MAX * 8;   // + the lists
+    if (NP == 12) {
+      OSB_SMEM_ATTR_ONCE(k_match_tc_topk<12>, 227 * 1024);
+      k_match_tc_topk<12><<<grid, MT_THREADS, smem_tk, stream>>>(tmT, p, *tk);
+    } else {
+      OSB_SMEM_ATTR_ONCE(k_match_tc_topk<8>, 227 * 1024);
+      k_match_tc_topk<8><<<grid, MT_THREADS, smem_tk, stream>>>(tmT, p, *tk);
+    }
+  } else if (ce != nullptr) {
     const size_t smem_ce = smem + 2 * MT_M * 4 + (size_t)3 * ce->classes * 4;   // + terms, flags, histogram
     if (NP == 12) {
       OSB_SMEM_ATTR_ONCE(k_match_tc_ce<12>, 227 * 1024);
@@ -479,16 +586,25 @@ static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, cons
   return 0;
 }
 
-static int fill_match_tc(MatchTcParams &p, const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a,
-                         const float *sel_b, int c, const int64_t *inds_reverse, int64_t n_pts, int k_text, int normalize,
-                         void *scores_f16, int64_t *label, float *smax, void *feat_out_f16) {
-  p = MatchTcParams{};
+static MatchTcParams match_tc_params(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a,
+                                     const float *sel_b, int c, const int64_t *inds_reverse, int64_t n_pts, int k_text,
+                                     int normalize, void *scores_f16, int64_t *label, float *smax, void *feat_out_f16) {
+  MatchTcParams p{};
   p.feat = feat; p.feat2 = (const __half *)feat2_f16; p.sel_a = sel_a; p.sel_b = sel_b;
   p.inds_reverse = inds_reverse; p.n_pts = n_pts; p.C = c; p.k_text = k_text;
   p.n_pass = (k_text + MT_NW - 1) / MT_NW;
-  OSB_CHECK(p.n_pass * MT_NW <= 512, "match: K_text=%d too large (at most 512 text rows)", k_text);
   p.feat_is_f16 = feat_is_f16; p.normalize = normalize;
   p.scores = (__half *)scores_f16; p.label = label; p.smax = smax; p.feat_out = (__half *)feat_out_f16;
+  return p;
+}
+
+// the [n_pts, K] epilogues: at most five passes
+static int fill_match_tc(MatchTcParams &p, const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a,
+                         const float *sel_b, int c, const int64_t *inds_reverse, int64_t n_pts, int k_text, int normalize,
+                         void *scores_f16, int64_t *label, float *smax, void *feat_out_f16) {
+  p = match_tc_params(feat, feat_is_f16, feat2_f16, sel_a, sel_b, c, inds_reverse, n_pts, k_text, normalize, scores_f16,
+                      label, smax, feat_out_f16);
+  OSB_CHECK(p.n_pass * MT_NW <= 512, "match: K_text=%d too large (at most 512 text rows)", k_text);
   return 0;
 }
 
@@ -499,7 +615,7 @@ int match_tc_run(const void *feat, int feat_is_f16, const void *feat2_f16, const
   if (fill_match_tc(p, feat, feat_is_f16, feat2_f16, sel_a, sel_b, c, inds_reverse, n_pts, k_text, normalize, scores_f16,
                     label, smax, feat_out_f16))
     return 1;
-  return launch_match_tc(p, nullptr, nullptr, text_f16, stream);
+  return launch_match_tc(p, nullptr, nullptr, nullptr, text_f16, stream);
 }
 
 int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
@@ -511,7 +627,7 @@ int match_tc_vote_run(const void *feat, int feat_is_f16, const void *feat2_f16, 
     return 1;
   const MatchTcVote vote{(__half *)store_f16, label_cur, label_acc,
                          (k_text % 2 == 0 && reinterpret_cast<uintptr_t>(store_f16) % 4 == 0) ? 1 : 0};
-  return launch_match_tc(p, &vote, nullptr, text_f16, stream);
+  return launch_match_tc(p, &vote, nullptr, nullptr, text_f16, stream);
 }
 
 int match_tc_ce_run(const void *feat, int feat_is_f16, int c, const int64_t *inds_reverse, int64_t n_pts, const void *text_f16,
@@ -527,7 +643,17 @@ int match_tc_ce_run(const void *feat, int feat_is_f16, int c, const int64_t *ind
                     nullptr, nullptr))
     return 1;
   const MatchTcCe ce{label, label_is_i64, ignore, classes, (double *)ws, (unsigned long long *)areas, bad, loss_f16};
-  return launch_match_tc(p, nullptr, &ce, text_f16, stream);
+  return launch_match_tc(p, nullptr, &ce, nullptr, text_f16, stream);
+}
+
+// streaming top-k: any number of passes (the caller bounds K)
+int match_tc_topk_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
+                      const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize, int topk,
+                      void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, cudaStream_t stream) {
+  const MatchTcParams p = match_tc_params(feat, feat_is_f16, feat2_f16, sel_a, sel_b, c, inds_reverse, n_pts, k_text,
+                                          normalize, nullptr, nullptr, smax, feat_out_f16);
+  const MatchTcTopk tk{topk, (__half *)scores_f16, label};
+  return launch_match_tc(p, nullptr, nullptr, &tk, text_f16, stream);
 }
 
 }  // namespace osb
