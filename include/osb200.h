@@ -454,6 +454,28 @@ int osb_match_ensemble_topk(const float *feat3d, const void *feat2d_f16, int64_t
                             const void *text_f16, int32_t k_text, int32_t topk, void *scores_f16, int64_t *label,
                             void *feat_out_f16, void *stream);
 
+/* Scene search (DESIGN.md, "Scene search contract"): fp16 rows [n_rows, c] of scenes stored one after another (scene s
+ * owns rows [scene_off[s], scene_off[s+1]); row_scene[r] int32 is the scene of row r) against fp16 queries [nq, c].  The
+ * scores are the bits osb_match_scores(rows, feat_is_f16 = 1, normalize = 0, inds_reverse = NULL, text = queries) writes;
+ * nothing of size [n_rows, nq] is written.  Order: NaN never ranks, is never a maximum and is never counted; numbers by
+ * descending value, -0 == +0; equal values to the lower global row.
+ *   top_score_f16 fp16 / top_scene int64 / top_row int64 [nq, k]: the k best rows per query, best first (top_row is the
+ *                  row within its scene); slots past the last non-NaN row are (-inf, -1, -1)
+ *   scene_max_f16 fp16 / scene_argmax int64 [n_scenes, nq]: the best score of each scene (its own bits) and its row within
+ *                  the scene, the lowest on ties; (-inf, -1) when the scene has no non-NaN score
+ *   scene_count int64 [n_scenes, nq] (may be NULL; needs threshold, fp32 [nq]): rows with float(s) >= threshold[q]
+ * scene_off_host (host memory) and scene_off (device) hold the same n_scenes + 1 offsets; the host copy is checked to
+ * run strictly increasing from 0 to n_rows.  1 <= nq <= OSB_SEARCH_MAX_QUERIES, 1 <= k <= OSB_SEARCH_MAX_K,
+ * 1 <= n_rows < 2^31; rows and queries 16-byte aligned.  The workspace (osb_search_workspace_bytes, 8-byte aligned,
+ * independent of n_rows) is overwritten.  A memset and two launches; two calls on the same inputs give the same bits. */
+#define OSB_SEARCH_MAX_QUERIES 96
+#define OSB_SEARCH_MAX_K 32
+size_t osb_search_workspace_bytes(int64_t n_scenes, int32_t nq, int32_t k);
+int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
+               const int64_t *scene_off, int64_t n_scenes, const void *queries_f16, int32_t nq, int32_t k,
+               const float *threshold, void *top_score_f16, int64_t *top_scene, int64_t *top_row, void *scene_max_f16,
+               int64_t *scene_argmax, int64_t *scene_count, void *ws, size_t ws_bytes, void *stream);
+
 /* Optional folded head (engine.forward_scores): rows z = [x L | x U] (fp32, row pitch ld floats) from one 1x1x1
  * convolution with the weights [L | U], W W^T = L L^T, U = W T^T  ->  score_k = fp16((x.U_k) / (|x L| + 1e-5)),
  * label = first argmax.  Same cosine scores as run/evaluate.py:305-310 without materialising the 768-d features. */

@@ -25,32 +25,12 @@
 // k_match_tc_topk is the same kernel with a running per-point top-k (k <= 8) in the epilogue (MatchTcTopk below), so the
 // number of passes has no bound of its own: the result is [N_pts, k], never [N_pts, K].  The three kernels above compile
 // to the same instructions as before it existed.
+#include "match_tc.cuh"
 #include "metric.cuh"
-#include "tc_ptx.cuh"
 #include "vote.cuh"
 #include <algorithm>
 
 namespace osb {
-
-constexpr int MT_M = 128;
-constexpr int MT_NW = 96;            // text rows per MMA pass (N of the instruction)
-constexpr int MT_PW = 16;             // A-producer warps (8 rows each)
-constexpr int MT_THREADS = (MT_PW + 1) * 32;   // + TMA warp
-constexpr int MT_BSTAGES = 2;
-
-struct MatchTcParams {
-  const void *feat;                  // [n_vox, C] fp32 or fp16
-  const __half *feat2;               // optional second source (fp16) for the ensemble select
-  const float *sel_a, *sel_b;        // ensemble: use feat2 where sel_a[p] < sel_b[p]
-  const int64_t *inds_reverse;       // [n_pts] or NULL
-  int64_t n_pts;
-  int C, k_text, n_pass;
-  int feat_is_f16, normalize;
-  __half *scores;                    // [n_pts, k_text] or NULL
-  int64_t *label;                    // [n_pts] or NULL
-  float *smax;                       // [n_pts] or NULL
-  __half *feat_out;                  // [n_pts, C] or NULL: the fp16 operand actually multiplied (ensemble feature)
-};
 
 // Test-time repeat vote (k_match_tc_vote): store[p,k] = fp16_rn(store[p,k] + scores[p,k]) in place, and the labels of
 // this repeat's scores and of the accumulated sum (vote.cuh: torch CPU `max(1)[1]`, NaN-first).
@@ -88,22 +68,6 @@ struct MatchTcTopk {
 constexpr int MT_TOPK_MAX = 8;
 
 enum { MT_PLAIN = 0, MT_VOTE = 1, MT_CE = 2, MT_TOPK = 3 };
-
-// order key of score h at column k: larger is better.  Bits 48-63 map the score to an unsigned order (NaN highest, -0 as
-// +0), bits 16-47 hold ~k (the lower column wins a tie), bits 0-15 the score's own fp16 bits.  Every valid key is > 0.
-__device__ __forceinline__ uint64_t topk_key(__half h, int k) {
-  const uint32_t b = __half_as_ushort(h);
-  const uint32_t u = (b & 0x7fffu) > 0x7c00u ? 0xffffu : b == 0x8000u ? 0x8000u : (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
-  return ((uint64_t)u << 48) | ((uint64_t)(~(uint32_t)k) << 16) | b;
-}
-
-// insert key into the descending list L[0..n) unless it is below L[n-1] (keys are distinct: one per column)
-__device__ __forceinline__ void topk_insert(uint64_t *L, int n, uint64_t key) {
-  if (key < L[n - 1]) return;
-  int j = n - 1;
-  for (; j > 0 && L[j - 1] < key; --j) L[j] = L[j - 1];
-  L[j] = key;
-}
 
 // the label of point row pt as an int: y in [0, K), ignore, or (a label outside [0, K)) a negative value other than ignore
 __device__ __forceinline__ int ce_label(const MatchTcCe &ce, int64_t pt, int64_t n_pts, int k_text) {
@@ -150,80 +114,7 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
 
   if (warp < MT_PW) {
     // ============================ A producers: 8 rows per warp ==============================
-    // RB rows are in flight per warp (their loads are issued before any is consumed): 16 warps x RB x 3 KB of
-    // outstanding loads per SM keeps HBM busy from the single resident CTA; 16 warps also spread the
-    // convert / normalise instruction stream over all four schedulers.
-    constexpr int RB = 2, ROWS_PW = MT_M / MT_PW;
-    for (int rr0 = 0; rr0 < ROWS_PW; rr0 += RB) {
-      float v[RB][2 * NP];
-      bool f16[RB], live[RB];
-      float ss[RB];
-#pragma unroll
-      for (int u = 0; u < RB; ++u) {
-        const int64_t pt = row0 + warp * ROWS_PW + rr0 + u;
-        live[u] = pt < p.n_pts;
-        f16[u] = false;
-        ss[u] = 0.f;
-        if (live[u]) {
-          const int64_t vox = p.inds_reverse ? __ldg(p.inds_reverse + pt) : pt;
-          bool second = false;
-          if (p.feat2 != nullptr) second = (p.sel_a == nullptr) ? true : (__ldg(p.sel_a + pt) < __ldg(p.sel_b + pt));
-          f16[u] = second || p.feat_is_f16;
-          const void *src = second ? (const void *)p.feat2 : p.feat;
-          if (f16[u]) {
-            const __half2 *q = reinterpret_cast<const __half2 *>(src) + vox * (C / 2);
-#pragma unroll
-            for (int j = 0; j < NP; ++j) {
-              const float2 f = __half22float2(__ldg(q + lane + 32 * j));
-              v[u][2 * j] = f.x; v[u][2 * j + 1] = f.y;
-            }
-          } else {
-            const float2 *q = reinterpret_cast<const float2 *>(src) + vox * (C / 2);
-#pragma unroll
-            for (int j = 0; j < NP; ++j) {
-              const float2 f = __ldg(q + lane + 32 * j);
-              v[u][2 * j] = f.x; v[u][2 * j + 1] = f.y;
-            }
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 2 * NP; ++j) v[u][j] = 0.f;
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < RB; ++u) {
-        const int r = warp * ROWS_PW + rr0 + u;
-        const int64_t pt = row0 + r;
-        if (p.normalize) {
-#pragma unroll
-          for (int j = 0; j < 2 * NP; ++j) ss[u] = fmaf(v[u][j], v[u][j], ss[u]);
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) ss[u] += __shfl_xor_sync(0xffffffffu, ss[u], o);
-          float nrm = sqrtf(ss[u]);
-          float d;
-          if (f16[u]) {   // the reference takes norm, +1e-5 and the division on an fp16 tensor (evaluate.py:303-305)
-            nrm = __half2float(__float2half_rn(nrm));
-            d = __half2float(__float2half_rn(nrm + 1e-5f));
-          } else {
-            d = nrm + 1e-5f;
-          }
-          // x / d evaluated as x * (1/d) (one rounding more than the reference's division; the following fp16
-          // rounding absorbs it except for values within 2^-24 of an fp16 rounding boundary)
-          const float rd = __frcp_rn(d);
-#pragma unroll
-          for (int j = 0; j < 2 * NP; ++j) v[u][j] = v[u][j] * rd;
-        }
-        // chunk j of this row: lane holds elements 2*lane, 2*lane+1 -> bytes [4*lane, 4*lane+4) of the 128-byte line
-        const uint32_t line = smem_u32(sA) + r * 128 + ((((4 * lane) >> 4) ^ (r & 7)) << 4) + ((4 * lane) & 15);
-#pragma unroll
-        for (int j = 0; j < NP; ++j) {
-          const __half2 h = __floats2half2_rn(v[u][2 * j], v[u][2 * j + 1]);       // the reference's `.half()`
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(line + j * (MT_M * 128)), "r"(*reinterpret_cast<const uint32_t *>(&h)) : "memory");
-          if (p.feat_out != nullptr && live[u])
-            reinterpret_cast<__half2 *>(p.feat_out)[pt * (C / 2) + lane + 32 * j] = h;
-        }
-      }
-    }
+    mt_fill_a<NP>(p, sA, row0, warp, lane);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic-proxy writes -> wgmma reads
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a_full) : "memory");
   } else if (warp == MT_PW) {

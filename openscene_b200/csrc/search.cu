@@ -1,0 +1,317 @@
+// Scene search (DESIGN.md, "Scene search contract"): a few query embeddings against every row of a database of scenes.
+//
+//   s[r, q] = fp16( sum_c A[r, c] * Q[q, c] )      the bits osb_match_scores writes for fp16 rows, normalize = 0
+//
+// Per query the k best rows of the whole index, and per scene and query the best score, its row and the number of rows
+// scoring at or above a threshold.  The [N, nq] scores never reach memory.
+//
+// k_search is a persistent loop over 128-row tiles (one CTA per SM).  Per tile, the A producers of the tensor-core match
+// (match_tc.cuh) load the rows and write the K-major operand, warp 16 streams the query chunks with TMA, and warps 0-7 run
+// the match kernel's wgmma pass and round to fp16.  The tile's fp16 scores then go to shared memory (over the A tile, which
+// the product no longer needs), and four threads per query scan a column each over 32 rows:
+//   - each run of one scene folds into (max order key, count); a tile inside one scene costs one 64-bit atomicMax and one
+//     integer add per query, a tile that crosses scenes one per run and quarter;
+//   - keys above the k-th key of the CTA's running list (global, L2-resident) are inserted into it, one lane of the
+//     quad at a time.
+// While the tile is multiplied and scanned, the producers have already asked L2 for the next tile's rows.
+// k_search_finish merges the per-CTA lists into the k best keys per query and decodes keys into (score, scene, row), and
+// decodes the per-scene keys and counts.
+//
+// Order key (search_key): bits 48-63 the score's order (-0 as +0), bits 16-47 ~row (the lower global row wins a tie), bits
+// 0-15 the score's fp16 bits; NaN has key 0, below every other key, so it never ranks, is never a maximum and is never
+// counted.  Keys are distinct, so the top-k is a function of the scores alone, and atomicMax / integer adds make the
+// per-scene results independent of the order in which CTAs arrive.
+#include "match_tc.cuh"
+#include <algorithm>
+
+namespace osb {
+
+constexpr int SR_LD = MT_NW + 8;           // fp16 score tile: row stride in halves
+constexpr int SR_MAX_GRID = 132;           // CTAs: one per SM of an H100 SXM at most (the workspace is sized for it)
+
+struct SearchParams {
+  MatchTcParams a;                         // the operand: fp16 rows, no gather, no normalisation
+  const int32_t *row_scene;                // [n] scene of every row
+  int64_t n, n_tiles;
+  int nq, k;
+  const float *thr;                        // [nq] or NULL (nothing counted)
+  uint64_t *lists;                         // [gridDim.x][nq][k] running top-k keys, descending
+  unsigned long long *scene_key;           // [S][nq] max key, 0 = none
+  unsigned long long *scene_cnt;           // [S][nq]
+};
+
+__device__ __forceinline__ uint64_t search_key(__half h, int64_t row) {
+  const uint32_t b = __half_as_ushort(h);
+  if ((b & 0x7fffu) > 0x7c00u) return 0;
+  const uint32_t u = b == 0x8000u ? 0x8000u : (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
+  return ((uint64_t)u << 48) | ((uint64_t)(~(uint32_t)row) << 16) | b;
+}
+
+__device__ __forceinline__ void scene_flush(const SearchParams &sp, int s, int q, uint64_t key, uint32_t cnt) {
+  if (s < 0) return;
+  const size_t i = (size_t)s * sp.nq + q;
+  if (key) atomicMax(sp.scene_key + i, (unsigned long long)key);
+  if (cnt) atomicAdd(sp.scene_cnt + i, (unsigned long long)cnt);
+}
+
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+template <int NP>
+__global__ void __launch_bounds__(MT_THREADS, 1) k_search(const __grid_constant__ CUtensorMap tmQ, const SearchParams sp) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr int C = 64 * NP;
+  constexpr int A_BYTES = NP * MT_M * 128, B_BYTES = MT_NW * 128;
+  uint8_t *sA = smem, *sB = smem + A_BYTES;
+  uint64_t *bars = reinterpret_cast<uint64_t *>(sB + MT_BSTAGES * B_BYTES);   // b_full[2], b_empty[2]
+  int32_t *s_scene = reinterpret_cast<int32_t *>(sB + MT_BSTAGES * B_BYTES + 128);
+  __half *sS = reinterpret_cast<__half *>(sA);                                 // [128][SR_LD] once the product is done
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t b_full = smem_u32(bars), b_empty = smem_u32(bars + 2);
+  uint64_t *lists = sp.lists + (size_t)blockIdx.x * sp.nq * sp.k;
+  if (tid == 0) {
+    for (int s = 0; s < MT_BSTAGES; ++s) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, 2); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (tid == MT_PW * 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQ) : "memory");
+  for (int i = tid; i < sp.nq * sp.k; i += MT_THREADS) lists[i] = 0;   // empty lists: key 0 is below every valid key
+  __syncthreads();
+
+  if (warp == MT_PW) {
+    // ============================ TMA producer: the query chunks of every tile ============================
+    int s = 0; uint32_t phase = 0;
+    for (int64_t t = blockIdx.x; t < sp.n_tiles; t += gridDim.x)
+      for (int c = 0; c < NP; ++c) mt_text_stage(tmQ, sB, b_full, b_empty, c, 0, s, phase);
+    return;
+  }
+
+  // warps 0-15 from here on; they synchronise on named barrier 1
+  int s = 0; uint32_t phase = 0;
+  for (int64_t t = blockIdx.x; t < sp.n_tiles; t += gridDim.x) {
+    const int64_t row0 = t * MT_M;
+    const int nrows = (int)std::min<int64_t>(MT_M, sp.n - row0);
+    {   // the next tile's rows into L2 while this one is loaded, multiplied and scanned
+      const int64_t nt = t + gridDim.x;
+      if (nt < sp.n_tiles) {
+        const char *base = reinterpret_cast<const char *>(sp.a.feat) + nt * MT_M * (int64_t)(2 * C);
+        const int64_t bytes = std::min<int64_t>(MT_M, sp.n - nt * MT_M) * (2 * C);
+        for (int64_t o = (int64_t)tid * 128; o < bytes; o += MT_PW * 32 * 128)
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(base + o));
+      }
+    }
+    if (tid < MT_M) s_scene[tid] = tid < nrows ? __ldg(sp.row_scene + row0 + tid) : -1;
+    mt_fill_a<NP>(sp.a, sA, row0, warp, lane);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic-proxy writes -> wgmma reads
+    bar_sync(1, MT_PW * 32);
+
+    if (warp < 8) {
+      // ============ wgmma: warpgroup g multiplies rows [64g, 64g + 64) by the query block; fp16 scores to sS ============
+      const int g = warp >> 2;
+      float acc[MT_NW / 2];
+#pragma unroll
+      for (int i = 0; i < MT_NW / 2; ++i) acc[i] = 0.f;
+      mt_mma_pass<NP>(acc, sA, sB, g, tid, b_full, b_empty, s, phase);
+      bar_sync(2, 256);                                                    // both warpgroups are done reading sA
+      const int r_lo = 64 * g + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < MT_NW / 8; ++i)
+          *reinterpret_cast<__half2 *>(sS + (r_lo + 8 * h) * SR_LD + 8 * i + cq) =
+              __floats2half2_rn(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+    }
+    bar_sync(1, MT_PW * 32);
+
+    if (tid < 4 * MT_NW) {
+      // ============ column scan: query q = tid / 4, rows 32 qu .. 32 qu + 31 (qu = tid % 4) ============
+      const int q = tid >> 2, qu = tid & 3;
+      const bool act = q < sp.nq;
+      const int first = s_scene[0];
+      const bool one = first == s_scene[nrows - 1];                        // scene ids ascend with the row
+      const float th = (act && sp.thr) ? __ldg(sp.thr + q) : __int_as_float(0x7fc00000);
+      uint64_t *L = lists + (size_t)(act ? q : 0) * sp.k;
+      const uint64_t kth = act ? L[sp.k - 1] : ~0ull;
+      uint64_t mk = 0;
+      uint32_t cnt = 0, cand = 0;
+      int cur = -1;
+      if (act) {
+        for (int j = 0; j < 32; ++j) {
+          const int r = 32 * qu + j;
+          if (r >= nrows) break;
+          const int sc = s_scene[r];
+          const __half h = sS[r * SR_LD + q];
+          const uint64_t key = search_key(h, row0 + r);
+          if (sc != cur) { scene_flush(sp, cur, q, mk, cnt); cur = sc; mk = 0; cnt = 0; }
+          mk = std::max(mk, key);
+          cnt += __half2float(h) >= th ? 1u : 0u;
+          if (key > kth) cand |= 1u << j;
+        }
+      }
+      if (one) {   // one scene: merge the quad, one update per query
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {
+          mk = std::max(mk, (uint64_t)__shfl_xor_sync(0xffffffffu, (unsigned long long)mk, o));
+          cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        }
+        if (qu == 0 && act) scene_flush(sp, first, q, mk, cnt);
+      } else if (act) {
+        scene_flush(sp, cur, q, mk, cnt);
+      }
+      if (__any_sync(0xffffffffu, cand != 0)) {   // the candidates, one lane of each quad at a time
+#pragma unroll 1
+        for (int w = 0; w < 4; ++w) {
+          if (qu == w) {
+            while (cand) {
+              const int j = __ffs(cand) - 1;
+              cand &= cand - 1;
+              const int r = 32 * qu + j;
+              topk_insert(L, sp.k, search_key(sS[r * SR_LD + q], row0 + r));
+            }
+          }
+          __syncwarp();
+        }
+      }
+    }
+    bar_sync(1, MT_PW * 32);                                               // sS is read: the next tile may overwrite it
+  }
+}
+
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = std::max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// blocks 0 .. nq-1: the k best keys of query q over all CTA lists, decoded; the other blocks: the per-scene results
+__global__ void __launch_bounds__(256)
+k_search_finish(const uint64_t *__restrict__ lists, int n_lists, int nq, int k, const int32_t *__restrict__ row_scene,
+                const int64_t *__restrict__ off, __half *top_score, int64_t *top_scene, int64_t *top_row,
+                const unsigned long long *__restrict__ scene_key, const unsigned long long *__restrict__ scene_cnt,
+                int64_t n_scenes, __half *scene_max, int64_t *scene_argmax, int64_t *scene_count) {
+  const int tid = threadIdx.x;
+  if ((int)blockIdx.x < nq) {
+    extern __shared__ uint64_t s_keys[];
+    __shared__ unsigned long long s_red[8];
+    const int q = blockIdx.x, n = n_lists * k;
+    for (int i = tid; i < n; i += 256) s_keys[i] = lists[((size_t)(i / k) * nq + q) * k + i % k];
+    __syncthreads();
+    uint64_t last = ~0ull;
+    for (int j = 0; j < k; ++j) {   // round j: the largest key below the previous one (keys are distinct)
+      unsigned long long m = 0;
+      for (int i = tid; i < n; i += 256) {
+        const uint64_t v = s_keys[i];
+        if (v < last && v > m) m = v;
+      }
+      m = warp_max_u64(m);
+      if ((tid & 31) == 0) s_red[tid >> 5] = m;
+      __syncthreads();
+      m = s_red[0];
+      for (int w = 1; w < 8; ++w) m = std::max(m, s_red[w]);
+      __syncthreads();
+      last = m;
+      if (tid == 0) {
+        const size_t o = (size_t)q * k + j;
+        if (m == 0) {   // fewer than k rows with a score
+          top_score[o] = __ushort_as_half((unsigned short)0xfc00u);
+          top_scene[o] = -1;
+          top_row[o] = -1;
+        } else {
+          const int64_t grow = (int64_t)(~(uint32_t)(m >> 16));
+          const int sc = row_scene[grow];
+          top_score[o] = __ushort_as_half((unsigned short)(m & 0xffffu));
+          top_scene[o] = sc;
+          top_row[o] = grow - off[sc];
+        }
+      }
+    }
+    return;
+  }
+  const int64_t total = n_scenes * nq, stride = (int64_t)(gridDim.x - nq) * 256;
+  for (int64_t i = (int64_t)(blockIdx.x - nq) * 256 + tid; i < total; i += stride) {
+    const uint64_t key = scene_key[i];
+    if (key == 0) {
+      scene_max[i] = __ushort_as_half((unsigned short)0xfc00u);
+      scene_argmax[i] = -1;
+    } else {
+      scene_max[i] = __ushort_as_half((unsigned short)(key & 0xffffu));
+      scene_argmax[i] = (int64_t)(~(uint32_t)(key >> 16)) - off[i / nq];
+    }
+    if (scene_count) scene_count[i] = (int64_t)scene_cnt[i];
+  }
+}
+
+}  // namespace osb
+
+using namespace osb;
+
+extern "C" {
+
+size_t osb_search_workspace_bytes(int64_t n_scenes, int32_t nq, int32_t k) {
+  if (n_scenes < 1 || nq < 1 || nq > OSB_SEARCH_MAX_QUERIES || k < 1 || k > OSB_SEARCH_MAX_K) return 0;
+  return (size_t)SR_MAX_GRID * nq * k * 8 + (size_t)2 * n_scenes * nq * 8;
+}
+
+int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
+               const int64_t *scene_off, int64_t n_scenes, const void *queries_f16, int32_t nq, int32_t k,
+               const float *threshold, void *top_score_f16, int64_t *top_scene, int64_t *top_row, void *scene_max_f16,
+               int64_t *scene_argmax, int64_t *scene_count, void *ws, size_t ws_bytes, void *stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  OSB_CHECK(c == 512 || c == 768, "osb_search: feature width %d unsupported (OpenScene uses 512 / 768)", c);
+  OSB_CHECK(nq >= 1 && nq <= OSB_SEARCH_MAX_QUERIES, "osb_search: nq=%d outside 1..%d", nq, OSB_SEARCH_MAX_QUERIES);
+  OSB_CHECK(k >= 1 && k <= OSB_SEARCH_MAX_K, "osb_search: k=%d outside 1..%d", k, OSB_SEARCH_MAX_K);
+  OSB_CHECK(n_rows >= 1 && n_rows < (int64_t(1) << 31), "osb_search: N=%lld outside 1..2^31-1", (long long)n_rows);
+  OSB_CHECK(n_scenes >= 1 && n_scenes <= n_rows, "osb_search: %lld scenes for %lld rows", (long long)n_scenes,
+            (long long)n_rows);
+  OSB_CHECK(rows_f16 && row_scene && scene_off_host && scene_off && queries_f16,
+            "osb_search: NULL rows, row scenes, scene offsets or queries");
+  OSB_CHECK(top_score_f16 && top_scene && top_row && scene_max_f16 && scene_argmax,
+            "osb_search: NULL top-k or per-scene output");
+  OSB_CHECK(scene_count == nullptr || threshold != nullptr, "osb_search: scene counts need a threshold");
+  OSB_CHECK(((uintptr_t)rows_f16 & 15) == 0 && ((uintptr_t)queries_f16 & 15) == 0,
+            "osb_search: rows and queries must be 16-byte aligned");
+  OSB_CHECK(scene_off_host[0] == 0 && scene_off_host[n_scenes] == n_rows,
+            "osb_search: scene offsets must run from 0 to N=%lld", (long long)n_rows);
+  for (int64_t s = 0; s < n_scenes; ++s)
+    OSB_CHECK(scene_off_host[s] < scene_off_host[s + 1], "osb_search: scene offsets not strictly increasing at scene %lld",
+              (long long)s);
+  const size_t need = osb_search_workspace_bytes(n_scenes, nq, k);
+  OSB_CHECK(ws != nullptr && ws_bytes >= need && ((uintptr_t)ws & 7) == 0,
+            "osb_search: 8-byte aligned workspace of %zu bytes required (got %zu)", need, ws_bytes);
+
+  const int64_t n_tiles = ceil_div(n_rows, MT_M);
+  int dev = 0, sms = SR_MAX_GRID;
+  OSB_CUDA(cudaGetDevice(&dev));
+  OSB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int grid = (int)std::min<int64_t>(n_tiles, std::min(sms, SR_MAX_GRID));
+
+  SearchParams sp{};
+  sp.a.feat = rows_f16; sp.a.feat_is_f16 = 1; sp.a.n_pts = n_rows; sp.a.C = c; sp.a.k_text = nq; sp.a.n_pass = 1;
+  sp.row_scene = row_scene; sp.n = n_rows; sp.n_tiles = n_tiles; sp.nq = nq; sp.k = k;
+  sp.thr = scene_count ? threshold : nullptr;
+  sp.lists = reinterpret_cast<uint64_t *>(ws);
+  sp.scene_key = reinterpret_cast<unsigned long long *>(sp.lists + (size_t)SR_MAX_GRID * nq * k);
+  sp.scene_cnt = sp.scene_key + (size_t)n_scenes * nq;
+  OSB_CUDA(cudaMemsetAsync(sp.scene_key, 0, (size_t)2 * n_scenes * nq * 8, stream));
+
+  CUtensorMap tmQ;
+  if (make_tmap_2b(&tmQ, queries_f16, (uint64_t)c, (uint64_t)nq, MT_NW, 1)) return 1;
+  const int NP = c / 64;
+  const size_t smem = (size_t)NP * MT_M * 128 + MT_BSTAGES * MT_NW * 128 + 128 + MT_M * 4 + 1024;
+  if (NP == 12) {
+    OSB_SMEM_ATTR_ONCE(k_search<12>, 227 * 1024);
+    k_search<12><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  } else {
+    OSB_SMEM_ATTR_ONCE(k_search<8>, 227 * 1024);
+    k_search<8><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  }
+  OSB_LAUNCH_CHECK();
+  const int scene_blocks = (int)std::min<int64_t>(ceil_div(n_scenes * nq, 256), 1024);
+  k_search_finish<<<nq + scene_blocks, 256, (size_t)grid * k * 8, stream>>>(
+      sp.lists, grid, nq, k, row_scene, scene_off, (__half *)top_score_f16, top_scene, top_row, sp.scene_key, sp.scene_cnt,
+      n_scenes, (__half *)scene_max_f16, scene_argmax, scene_count);
+  OSB_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // extern "C"
