@@ -476,6 +476,42 @@ int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, i
                const float *threshold, void *top_score_f16, int64_t *top_scene, int64_t *top_row, void *scene_max_f16,
                int64_t *scene_argmax, int64_t *scene_count, void *ws, size_t ws_bytes, void *stream);
 
+/* Regions of search hits (DESIGN.md, "Region contract").  A hit is a (row, query) with float(s[r, q]) >= threshold[q], s the
+ * bits osb_search scores; NaN is never a hit.
+ *
+ * osb_search_hits: the hit list of one launch of at most OSB_SEARCH_MAX_QUERIES queries, sorted by (query, global row).
+ *   scene_count  int64 [n_scenes, nq]: osb_search's counts for the same rows, queries and threshold; n_hits their sum
+ *   hit_key      out int64 [n_hits]: (query << 32) | global row, ascending
+ *   hit_score_f16 out fp16 [n_hits]: s[row, query]
+ *   status       int32, or-ed with OSB_REGIONS_ST_COUNT when a (query, scene) segment does not receive exactly its count
+ * Arguments as osb_search; the workspace is osb_search_hits_workspace_bytes (8-byte aligned). */
+#define OSB_REGIONS_ST_COUNT 1    /* emitted hits differ from the counts */
+#define OSB_REGIONS_ST_RANGE 2    /* a hit's coordinate lies outside |x|, |y|, |z| < 2^17 - 256 */
+#define OSB_REGIONS_ST_DUP 4      /* two hits of one (scene, query) share a voxel */
+#define OSB_REGIONS_MAX_R 32
+size_t osb_search_hits_workspace_bytes(int64_t n_scenes, int32_t nq, int64_t n_hits);
+int osb_search_hits(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
+                    int64_t n_scenes, const void *queries_f16, int32_t nq, const float *threshold,
+                    const int64_t *scene_count, int64_t n_hits, int64_t *hit_key, void *hit_score_f16, int32_t *status,
+                    void *ws, size_t ws_bytes, void *stream);
+/* osb_regions: connected components of the hits of each (scene, query) under Chebyshev distance <= reach (1 or 2) on the
+ * int32 coordinates coords [n_rows, 4] = (x, y, z, unused), and the R best per query of those with at least min_voxels
+ * voxels, ranked by the search key of their best hit.  n_hits may be 0 (everything padded).
+ *   score_f16 fp16 / scene int64 / row int64 / size int64 [nq, R], box_min / box_max int32 [nq, R, 3]: unused slots
+ *             (-inf, -1, -1, 0, 0, 0)
+ *   n_regions int64 [n_scenes, nq]: regions with at least min_voxels voxels
+ *   hit_query / hit_scene / hit_row / hit_region int64 [n_hits] (all four or none): per hit in list order, hit_region the
+ *             rank of its region in its query's list or -1
+ *   status    or-ed with OSB_REGIONS_ST_RANGE / OSB_REGIONS_ST_DUP (duplicates among hits only)
+ * 1 <= nq <= OSB_SEARCH_MAX_QUERIES, 1 <= R <= OSB_REGIONS_MAX_R, min_voxels >= 1; coords 16-byte aligned; the workspace is
+ * osb_regions_workspace_bytes (8-byte aligned).  Integer atomics only: two calls give the same bits. */
+size_t osb_regions_workspace_bytes(int64_t n_hits);
+int osb_regions(const int64_t *hit_key, const void *hit_score_f16, int64_t n_hits, const int32_t *coords,
+                const int32_t *row_scene, const int64_t *scene_off, int64_t n_rows, int64_t n_scenes, int32_t nq, int32_t R,
+                int32_t reach, int32_t min_voxels, void *score_f16, int64_t *scene, int64_t *row, int64_t *size,
+                int32_t *box_min, int32_t *box_max, int64_t *n_regions, int64_t *hit_query, int64_t *hit_scene,
+                int64_t *hit_row, int64_t *hit_region, int32_t *status, void *ws, size_t ws_bytes, void *stream);
+
 /* Optional folded head (engine.forward_scores): rows z = [x L | x U] (fp32, row pitch ld floats) from one 1x1x1
  * convolution with the weights [L | U], W W^T = L L^T, U = W T^T  ->  score_k = fp16((x.U_k) / (|x L| + 1e-5)),
  * label = first argmax.  Same cosine scores as run/evaluate.py:305-310 without materialising the 768-d features. */

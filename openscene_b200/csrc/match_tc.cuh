@@ -37,6 +37,15 @@ __device__ __forceinline__ uint64_t topk_key(__half h, int k) {
   return ((uint64_t)u << 48) | ((uint64_t)(~(uint32_t)k) << 16) | b;
 }
 
+// order key of the scene search (search.cu, regions.cu): bits 48-63 the score's order (-0 as +0), bits 16-47 ~row (the
+// lower global row wins a tie), bits 0-15 the score's fp16 bits; NaN has key 0, below every other key.
+__device__ __forceinline__ uint64_t search_key(__half h, int64_t row) {
+  const uint32_t b = __half_as_ushort(h);
+  if ((b & 0x7fffu) > 0x7c00u) return 0;
+  const uint32_t u = b == 0x8000u ? 0x8000u : (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
+  return ((uint64_t)u << 48) | ((uint64_t)(~(uint32_t)row) << 16) | b;
+}
+
 // insert key into the descending list L[0..n) unless it is below L[n-1] (keys are distinct: one per column)
 __device__ __forceinline__ void topk_insert(uint64_t *L, int n, uint64_t key) {
   if (key < L[n - 1]) return;

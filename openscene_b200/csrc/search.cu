@@ -22,6 +22,7 @@
 // counted.  Keys are distinct, so the top-k is a function of the scores alone, and atomicMax / integer adds make the
 // per-scene results independent of the order in which CTAs arrive.
 #include "match_tc.cuh"
+#include "sortscan.cuh"
 #include <algorithm>
 
 namespace osb {
@@ -38,14 +39,14 @@ struct SearchParams {
   uint64_t *lists;                         // [gridDim.x][nq][k] running top-k keys, descending
   unsigned long long *scene_key;           // [S][nq] max key, 0 = none
   unsigned long long *scene_cnt;           // [S][nq]
+  // hit emission (k_search<NP, true> only)
+  int64_t n_scenes;
+  unsigned long long *cursor;              // [nq][S] next free slot of each (query, scene) segment of the hit list
+  const unsigned long long *seg_end;       // [nq][S] end of each segment
+  uint64_t *hit_key;                       // [n_hits] (query << 32) | global row, in arrival order
+  __half *hit_score;                       // [n_hits]
+  int *status;                             // OSB_REGIONS_ST_COUNT when a segment's hits do not match its count
 };
-
-__device__ __forceinline__ uint64_t search_key(__half h, int64_t row) {
-  const uint32_t b = __half_as_ushort(h);
-  if ((b & 0x7fffu) > 0x7c00u) return 0;
-  const uint32_t u = b == 0x8000u ? 0x8000u : (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
-  return ((uint64_t)u << 48) | ((uint64_t)(~(uint32_t)row) << 16) | b;
-}
 
 __device__ __forceinline__ void scene_flush(const SearchParams &sp, int s, int q, uint64_t key, uint32_t cnt) {
   if (s < 0) return;
@@ -54,9 +55,29 @@ __device__ __forceinline__ void scene_flush(const SearchParams &sp, int s, int q
   if (cnt) atomicAdd(sp.scene_cnt + i, (unsigned long long)cnt);
 }
 
+// the hits of one scene run of a thread's 32 rows (bit j = row 32 qu + j) into their (query, scene) segment
+__device__ __forceinline__ void hit_flush(const SearchParams &sp, const __half *sS, int64_t row0, int qu, int q, int s,
+                                          uint32_t hm) {
+  if (hm == 0) return;
+  const size_t seg = (size_t)q * sp.n_scenes + s;
+  const uint32_t n = __popc(hm);
+  unsigned long long pos = atomicAdd(sp.cursor + seg, (unsigned long long)n);
+  if (pos + n > sp.seg_end[seg]) { atomicOr(sp.status, OSB_REGIONS_ST_COUNT); return; }
+  while (hm) {
+    const int j = __ffs(hm) - 1;
+    hm &= hm - 1;
+    const int r = 32 * qu + j;
+    sp.hit_key[pos] = ((uint64_t)q << 32) | (uint64_t)(row0 + r);
+    sp.hit_score[pos] = sS[r * SR_LD + q];
+    ++pos;
+  }
+}
+
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
-template <int NP>
+// HITS = false: the search epilogue below.  HITS = true: the same loads, query stream and product; the epilogue writes
+// every (row, query) with float(s) >= thr[q] into the hit list instead (osb_search_hits).
+template <int NP, bool HITS = false>
 __global__ void __launch_bounds__(MT_THREADS, 1) k_search(const __grid_constant__ CUtensorMap tmQ, const SearchParams sp) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -75,7 +96,8 @@ __global__ void __launch_bounds__(MT_THREADS, 1) k_search(const __grid_constant_
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (tid == MT_PW * 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQ) : "memory");
-  for (int i = tid; i < sp.nq * sp.k; i += MT_THREADS) lists[i] = 0;   // empty lists: key 0 is below every valid key
+  if constexpr (!HITS)
+    for (int i = tid; i < sp.nq * sp.k; i += MT_THREADS) lists[i] = 0;   // empty lists: key 0 is below every valid key
   __syncthreads();
 
   if (warp == MT_PW) {
@@ -123,7 +145,23 @@ __global__ void __launch_bounds__(MT_THREADS, 1) k_search(const __grid_constant_
     }
     bar_sync(1, MT_PW * 32);
 
-    if (tid < 4 * MT_NW) {
+    if constexpr (HITS) {
+      // ============ hit emission: query q = tid / 4, rows 32 qu .. 32 qu + 31, one segment cursor update per scene run ============
+      const int q = tid >> 2, qu = tid & 3;
+      if (tid < 4 * MT_NW && q < sp.nq) {
+        const float th = __ldg(sp.thr + q);
+        int cur = -1;
+        uint32_t hm = 0;
+        for (int j = 0; j < 32; ++j) {
+          const int r = 32 * qu + j;
+          if (r >= nrows) break;
+          const int sc = s_scene[r];
+          if (sc != cur) { if (cur >= 0) hit_flush(sp, sS, row0, qu, q, cur, hm); cur = sc; hm = 0; }
+          if (__half2float(sS[r * SR_LD + q]) >= th) hm |= 1u << j;
+        }
+        if (cur >= 0) hit_flush(sp, sS, row0, qu, q, cur, hm);
+      }
+    } else if (tid < 4 * MT_NW) {
       // ============ column scan: query q = tid / 4, rows 32 qu .. 32 qu + 31 (qu = tid % 4) ============
       const int q = tid >> 2, qu = tid & 3;
       const bool act = q < sp.nq;
@@ -241,6 +279,41 @@ k_search_finish(const uint64_t *__restrict__ lists, int n_lists, int nq, int k, 
   }
 }
 
+// segments of the hit list in (query, scene) order: base = exclusive scan of scene_count[s][q] over (q, s); one block
+__global__ void __launch_bounds__(1024)
+k_hit_segments(const int64_t *__restrict__ scene_count, int64_t n_scenes, int nq, int64_t n_hits,
+               unsigned long long *cursor, unsigned long long *seg_end, int *status) {
+  __shared__ unsigned long long s_part[1024];
+  const int64_t m = n_scenes * nq, per = (m + 1023) / 1024;
+  const int64_t a = std::min<int64_t>(m, per * threadIdx.x), b = std::min<int64_t>(m, a + per);
+  unsigned long long t = 0;
+  for (int64_t i = a; i < b; ++i) t += (unsigned long long)scene_count[(i % n_scenes) * nq + i / n_scenes];
+  s_part[threadIdx.x] = t;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long run = 0;
+    for (int i = 0; i < 1024; ++i) { const unsigned long long v = s_part[i]; s_part[i] = run; run += v; }
+    if (run != (unsigned long long)n_hits) atomicOr(status, OSB_REGIONS_ST_COUNT);
+  }
+  __syncthreads();
+  unsigned long long run = s_part[threadIdx.x];
+  for (int64_t i = a; i < b; ++i) {
+    cursor[i] = run;
+    run += (unsigned long long)scene_count[(i % n_scenes) * nq + i / n_scenes];
+    seg_end[i] = std::min<unsigned long long>(run, (unsigned long long)n_hits);
+  }
+}
+
+// every segment received exactly its count; the scores follow the sorted keys (payload = arrival slot)
+__global__ void k_hit_finish(const unsigned long long *__restrict__ cursor, const unsigned long long *__restrict__ seg_end,
+                             int64_t n_seg, const int32_t *__restrict__ slot, const __half *__restrict__ score_in,
+                             int64_t n_hits, __half *score_out, int *status) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_seg; i += stride)
+    if (cursor[i] != seg_end[i]) atomicOr(status, OSB_REGIONS_ST_COUNT);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_hits; i += stride) score_out[i] = score_in[slot[i]];
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -310,6 +383,89 @@ int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, i
   k_search_finish<<<nq + scene_blocks, 256, (size_t)grid * k * 8, stream>>>(
       sp.lists, grid, nq, k, row_scene, scene_off, (__half *)top_score_f16, top_scene, top_row, sp.scene_key, sp.scene_cnt,
       n_scenes, (__half *)scene_max_f16, scene_argmax, scene_count);
+  OSB_LAUNCH_CHECK();
+  return 0;
+}
+
+size_t osb_search_hits_workspace_bytes(int64_t n_scenes, int32_t nq, int64_t n_hits) {
+  if (n_scenes < 1 || nq < 1 || nq > OSB_SEARCH_MAX_QUERIES || n_hits < 1 || n_hits >= (int64_t(1) << 31)) return 0;
+  // arrival keys 8, two payloads 4 + 4, arrival scores 2 (rounded up to 8 B per 4 hits), two [nq][S] arrays, sort histogram
+  return (size_t)n_hits * 16 + (size_t)((n_hits + 3) / 4) * 8 + (size_t)2 * n_scenes * nq * 8 + radix_sort_ws_bytes(n_hits);
+}
+
+int osb_search_hits(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
+                    int64_t n_scenes, const void *queries_f16, int32_t nq, const float *threshold,
+                    const int64_t *scene_count, int64_t n_hits, int64_t *hit_key, void *hit_score_f16, int32_t *status,
+                    void *ws, size_t ws_bytes, void *stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  OSB_CHECK(c == 512 || c == 768, "osb_search_hits: feature width %d unsupported (OpenScene uses 512 / 768)", c);
+  OSB_CHECK(nq >= 1 && nq <= OSB_SEARCH_MAX_QUERIES, "osb_search_hits: nq=%d outside 1..%d", nq, OSB_SEARCH_MAX_QUERIES);
+  OSB_CHECK(n_rows >= 1 && n_rows < (int64_t(1) << 31), "osb_search_hits: N=%lld outside 1..2^31-1", (long long)n_rows);
+  OSB_CHECK(n_scenes >= 1 && n_scenes <= n_rows, "osb_search_hits: %lld scenes for %lld rows", (long long)n_scenes,
+            (long long)n_rows);
+  OSB_CHECK(n_hits >= 1 && n_hits < (int64_t(1) << 31), "osb_search_hits: n_hits=%lld outside 1..2^31-1",
+            (long long)n_hits);
+  OSB_CHECK(rows_f16 && row_scene && scene_off_host && queries_f16 && threshold && scene_count,
+            "osb_search_hits: NULL rows, row scenes, scene offsets, queries, threshold or scene counts");
+  OSB_CHECK(hit_key && hit_score_f16 && status, "osb_search_hits: NULL hit list or status");
+  OSB_CHECK(((uintptr_t)rows_f16 & 15) == 0 && ((uintptr_t)queries_f16 & 15) == 0,
+            "osb_search_hits: rows and queries must be 16-byte aligned");
+  OSB_CHECK(((uintptr_t)hit_key & 7) == 0 && ((uintptr_t)hit_score_f16 & 1) == 0 && ((uintptr_t)status & 3) == 0,
+            "osb_search_hits: misaligned hit list or status");
+  OSB_CHECK(scene_off_host[0] == 0 && scene_off_host[n_scenes] == n_rows,
+            "osb_search_hits: scene offsets must run from 0 to N=%lld", (long long)n_rows);
+  for (int64_t s = 0; s < n_scenes; ++s)
+    OSB_CHECK(scene_off_host[s] < scene_off_host[s + 1],
+              "osb_search_hits: scene offsets not strictly increasing at scene %lld", (long long)s);
+  const size_t need = osb_search_hits_workspace_bytes(n_scenes, nq, n_hits);
+  OSB_CHECK(ws != nullptr && ws_bytes >= need && ((uintptr_t)ws & 7) == 0,
+            "osb_search_hits: 8-byte aligned workspace of %zu bytes required (got %zu)", need, ws_bytes);
+
+  uint8_t *w = reinterpret_cast<uint8_t *>(ws);
+  uint64_t *keys_a = reinterpret_cast<uint64_t *>(w);                       w += (size_t)n_hits * 8;
+  int32_t *vals_a = reinterpret_cast<int32_t *>(w);                         w += (size_t)n_hits * 4;
+  int32_t *vals_b = reinterpret_cast<int32_t *>(w);                         w += (size_t)n_hits * 4;
+  __half *score_a = reinterpret_cast<__half *>(w);                          w += (size_t)((n_hits + 3) / 4) * 8;
+  unsigned long long *cursor = reinterpret_cast<unsigned long long *>(w);   w += (size_t)n_scenes * nq * 8;
+  unsigned long long *seg_end = reinterpret_cast<unsigned long long *>(w);  w += (size_t)n_scenes * nq * 8;
+  void *sort_ws = w;
+
+  k_hit_segments<<<1, 1024, 0, stream>>>(scene_count, n_scenes, nq, n_hits, cursor, seg_end, status);
+  OSB_LAUNCH_CHECK();
+
+  const int64_t n_tiles = ceil_div(n_rows, MT_M);
+  int dev = 0, sms = SR_MAX_GRID;
+  OSB_CUDA(cudaGetDevice(&dev));
+  OSB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int grid = (int)std::min<int64_t>(n_tiles, std::min(sms, SR_MAX_GRID));
+  SearchParams sp{};
+  sp.a.feat = rows_f16; sp.a.feat_is_f16 = 1; sp.a.n_pts = n_rows; sp.a.C = c; sp.a.k_text = nq; sp.a.n_pass = 1;
+  sp.row_scene = row_scene; sp.n = n_rows; sp.n_tiles = n_tiles; sp.nq = nq; sp.k = 1;
+  sp.thr = threshold;
+  sp.n_scenes = n_scenes; sp.cursor = cursor; sp.seg_end = seg_end; sp.hit_key = keys_a; sp.hit_score = score_a;
+  sp.status = status;
+  CUtensorMap tmQ;
+  if (make_tmap_2b(&tmQ, queries_f16, (uint64_t)c, (uint64_t)nq, MT_NW, 1)) return 1;
+  const int NP = c / 64;
+  const size_t smem = (size_t)NP * MT_M * 128 + MT_BSTAGES * MT_NW * 128 + 128 + MT_M * 4 + 1024;
+  if (NP == 12) {
+    OSB_SMEM_ATTR_ONCE((k_search<12, true>), 227 * 1024);
+    k_search<12, true><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  } else {
+    OSB_SMEM_ATTR_ONCE((k_search<8, true>), 227 * 1024);
+    k_search<8, true><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  }
+  OSB_LAUNCH_CHECK();
+
+  // canonical order: stable sort by (query << 32) | global row, distinct per hit (bits 0..38: q < 96, row < 2^31)
+  uint64_t *keys_out = reinterpret_cast<uint64_t *>(hit_key);
+  const int where = radix_sort_pairs(keys_a, vals_a, keys_out, vals_b, nullptr, n_hits, 0, 39, sort_ws, stream);
+  OSB_CHECK(where >= 0, "osb_search_hits: sort launch failed");
+  const int32_t *slot = where ? vals_b : vals_a;
+  if (where == 0) OSB_CUDA(cudaMemcpyAsync(keys_out, keys_a, (size_t)n_hits * 8, cudaMemcpyDeviceToDevice, stream));
+  const int blocks = (int)std::min<int64_t>(ceil_div(std::max<int64_t>(n_hits, n_scenes * nq), 256), 4096);
+  k_hit_finish<<<blocks, 256, 0, stream>>>(cursor, seg_end, n_scenes * nq, slot, score_a, n_hits,
+                                           (__half *)hit_score_f16, status);
   OSB_LAUNCH_CHECK();
   return 0;
 }

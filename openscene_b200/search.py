@@ -10,6 +10,10 @@ fixed device arena, and ``query`` scores every row against the queries on the te
 
 The [N, nq] scores never exist in memory.  One memset and two launches serve up to 96 queries, and each such slice reads
 the index once; more queries run slice after slice.  Nothing synchronises the host.
+
+An index built with ``coords=True`` also keeps each row's voxel coordinates, and ``regions`` groups each query's hits
+(rows at or above a threshold) into spatially connected regions on the device (csrc/regions.cu; DESIGN.md, "Region
+contract"): the objects a search for a name or an image is after, with their boxes, sizes and best hits.
 """
 from collections import namedtuple
 
@@ -19,19 +23,30 @@ from . import _cabi as C
 
 MAX_QUERIES = 96      # OSB_SEARCH_MAX_QUERIES: one 96-column wgmma pass per launch
 MAX_K = 32            # OSB_SEARCH_MAX_K
+MAX_REGIONS = 32      # OSB_REGIONS_MAX_R
+C_ST_COUNT, C_ST_RANGE, C_ST_DUP = 1, 2, 4      # OSB_REGIONS_ST_*: the status word of osb_search_hits / osb_regions
 
 SearchResult = namedtuple('SearchResult', 'score scene row scene_max scene_argmax scene_count')
 SearchResult.__doc__ = """score fp16 / scene int64 / row int64 [nq, k]: best first, (-inf, -1, -1) past the last non-NaN row;
 scene_max fp16 / scene_argmax int64 [S, nq]: (-inf, -1) for a scene without a non-NaN score; scene_count int64 [S, nq]
 (rows with float(score) >= threshold[q]) or None."""
 
+RegionResult = namedtuple('RegionResult', 'score scene row size box_min box_max n_regions '
+                                          'hit_query hit_scene hit_row hit_score hit_region')
+RegionResult.__doc__ = """score fp16 / scene int64 / row int64 / size int64 [nq, R], box_min / box_max int32 [nq, R, 3]: the
+best regions per query, ranked by the search key of their best hit (score, scene and row within the scene of that hit);
+unused slots (-inf, -1, -1, 0, 0, 0).  n_regions int64 [S, nq]: regions of at least min_voxels voxels.  With hits=True,
+hit_query / hit_scene / hit_row int64, hit_score fp16 and hit_region int64 [n_hits] list every hit sorted by (query,
+global row), hit_region the rank of its region in its query's list or -1; otherwise None."""
+
 
 class SceneIndex:
     """A fixed device arena of fp16 operand rows [capacity_rows, channels], filled scene after scene by ``add``.
 
-    Scene ids follow the order of ``add``.  The arena never grows and is never re-copied."""
+    Scene ids follow the order of ``add``.  The arena never grows and is never re-copied.  With ``coords=True`` an int32
+    [capacity_rows, 4] arena holds each row's voxel coordinates (x, y, z, 0), which ``regions`` needs."""
 
-    def __init__(self, capacity_rows, channels=768, device=None):
+    def __init__(self, capacity_rows, channels=768, device=None, coords=False):
         if channels not in (512, 768):
             raise ValueError(f"SceneIndex: channels must be 512 or 768 (got {channels})")
         if not 1 <= capacity_rows < 2 ** 31:
@@ -45,6 +60,7 @@ class SceneIndex:
         self.channels = int(channels)
         self.rows = torch.empty((self.capacity, self.channels), dtype=torch.float16, device=self.device)
         self.row_scene = torch.empty(self.capacity, dtype=torch.int32, device=self.device)
+        self.coords = torch.zeros((self.capacity, 4), dtype=torch.int32, device=self.device) if coords else None
         self._off = [0]                                    # host offsets, n_scenes + 1
         self._off_dev = torch.zeros(64, dtype=torch.int64, device=self.device)
         self.names = []
@@ -61,10 +77,18 @@ class SceneIndex:
         """The rows [n, C] of one scene (a view into the arena)."""
         return self.rows[self._off[scene]:self._off[scene + 1]]
 
-    def add(self, rows, name=None):
+    def scene_coords(self, scene):
+        """The voxel coordinates [n, 4] (x, y, z, 0) of one scene, row for row with ``scene_rows`` (a view)."""
+        if self.coords is None:
+            raise RuntimeError("SceneIndex.scene_coords: the index was built without coordinates (coords=True)")
+        return self.coords[self._off[scene]:self._off[scene + 1]]
+
+    def add(self, rows, name=None, coords=None):
         """Append one scene's operand rows (fp16 [n, C]; fp32 is taken as ``.half()``, the 'distill' operand) and return
-        its scene id.  An empty scene, a wrong width, dtype or device, or a full arena is refused before anything is
-        copied."""
+        its scene id.  ``coords``: integer voxel coordinates [n, 3], or [n, 4] in MinkowskiEngine's (batch, x, y, z)
+        layout whose batch column is dropped, row for row with ``rows``; required on an index built with coordinates and
+        refused on one without.  An empty scene, a wrong width, dtype or device, or a full arena is refused before
+        anything is copied."""
         if not isinstance(rows, torch.Tensor) or rows.dim() != 2:
             raise ValueError("SceneIndex.add: rows must be a 2-D tensor [n, C]")
         if rows.dtype not in (torch.float16, torch.float32):
@@ -76,12 +100,27 @@ class SceneIndex:
             raise ValueError(f"SceneIndex.add: rows have width {c}, the index {self.channels}")
         if n < 1:
             raise ValueError("SceneIndex.add: empty scene")
+        if self.coords is None and coords is not None:
+            raise ValueError("SceneIndex.add: coordinates given to an index built without them (coords=True)")
+        if self.coords is not None:
+            if coords is None:
+                raise ValueError("SceneIndex.add: this index keeps coordinates; pass coords [n, 3] or [n, 4]")
+            if not isinstance(coords, torch.Tensor) or coords.dim() != 2 or coords.shape[1] not in (3, 4):
+                raise ValueError("SceneIndex.add: coords must be a 2-D tensor [n, 3] (x, y, z) or [n, 4] (batch, x, y, z)")
+            if coords.dtype not in (torch.int32, torch.int64, torch.int16, torch.uint8, torch.int8):
+                raise TypeError(f"SceneIndex.add: coords must be integer (got {coords.dtype})")
+            if coords.shape[0] != n:
+                raise ValueError(f"SceneIndex.add: {coords.shape[0]} coordinates for {n} rows")
+            if coords.device != self.device:
+                raise ValueError(f"SceneIndex.add: coords are on {coords.device}, the index on {self.device}")
         o = self.n_rows
         if o + n > self.capacity:
             raise RuntimeError(f"SceneIndex.add: {n} rows do not fit ({self.capacity - o} of {self.capacity} left)")
         s = self.n_scenes
         self.rows[o:o + n].copy_(rows)                    # fp32 -> fp16 rounds to nearest even, as `.half()`
         self.row_scene[o:o + n].fill_(s)
+        if self.coords is not None:
+            self.coords[o:o + n, :3].copy_(coords[:, -3:])
         if s + 2 > self._off_dev.numel():
             grown = torch.zeros(2 * self._off_dev.numel(), dtype=torch.int64, device=self.device)
             grown[:self._off_dev.numel()].copy_(self._off_dev)
@@ -128,6 +167,108 @@ class SceneIndex:
         return SearchResult(*(None if parts[0][j] is None else torch.cat([p[j] for p in parts], dim=0 if j < 3 else 1)
                               for j in range(6)))
 
+    def _queries(self, queries, what):
+        q = queries.to(device=self.device, dtype=torch.float16)
+        if q.dim() == 1:
+            q = q.unsqueeze(0)
+        if q.dim() != 2 or q.shape[1] != self.channels or q.shape[0] < 1:
+            raise ValueError(f"SceneIndex.{what}: queries must be [nq >= 1, {self.channels}] (got {tuple(queries.shape)})")
+        return q
+
+    def _thresholds(self, threshold, nq, what):
+        if isinstance(threshold, torch.Tensor):
+            thr = threshold.to(device=self.device, dtype=torch.float32).reshape(-1)
+        else:     # a number or a list: filled on the device, no copy that would wait for the host
+            vals = [float(threshold)] if isinstance(threshold, (int, float)) else [float(v) for v in threshold]
+            thr = torch.empty(len(vals), dtype=torch.float32, device=self.device)
+            if len(vals) == 1:
+                thr.fill_(vals[0])
+            else:
+                for i, v in enumerate(vals):
+                    thr[i] = v
+        if thr.numel() == 1:
+            thr = thr.expand(nq)
+        if thr.numel() != nq:
+            raise ValueError(f"SceneIndex.{what}: {thr.numel()} thresholds for {nq} queries")
+        return thr.contiguous()
+
+    def regions(self, queries, threshold, max_regions=8, reach=1, min_voxels=1, hits=False, max_hits=2 ** 26):
+        """Group each query's hits, the rows r with float(s[r, q]) >= threshold[q] (s the bits ``query`` scores), into
+        connected regions: two hits of one scene are adjacent when their coordinates differ by at most ``reach`` (1 or
+        2) on every axis.  Returns a ``RegionResult`` with the ``max_regions`` (1..32) best regions of at least
+        ``min_voxels`` voxels per query.  Any nq: slices of 96 queries.
+
+        Two host synchronisations: one read of the total hit count (from ``osb_search``'s counts), which sizes the hit
+        buffers and is refused above ``max_hits`` before they are allocated, and one read of a status word at the end,
+        which raises when a hit's coordinate lies outside |x|, |y|, |z| < 2^17 - 256 or two hits of one (scene, query)
+        share a voxel.  Duplicate coordinates among rows that are not hits are not inspected."""
+        if self.coords is None:
+            raise RuntimeError("SceneIndex.regions: the index was built without coordinates (coords=True)")
+        if self.n_scenes == 0:
+            raise RuntimeError("SceneIndex.regions: the index is empty")
+        if not 1 <= max_regions <= MAX_REGIONS:
+            raise ValueError(f"SceneIndex.regions: max_regions={max_regions} outside 1..{MAX_REGIONS}")
+        if reach not in (1, 2):
+            raise ValueError(f"SceneIndex.regions: reach={reach} outside 1..2")
+        if min_voxels < 1:
+            raise ValueError(f"SceneIndex.regions: min_voxels={min_voxels} below 1")
+        q = self._queries(queries, 'regions')
+        nq, S, dev, R = q.shape[0], self.n_scenes, self.device, int(max_regions)
+        thr = self._thresholds(threshold, nq, 'regions')
+        slices = [(i, q[i:i + MAX_QUERIES].contiguous(), thr[i:i + MAX_QUERIES].contiguous())
+                  for i in range(0, nq, MAX_QUERIES)]
+        counts = [self._query(qs, 1, ts).scene_count for _, qs, ts in slices]
+        with torch.cuda.device(dev):
+            totals = [int(t) for t in torch.stack([c.sum() for c in counts]).tolist()]      # host sync 1
+        total = sum(totals)
+        if total > max_hits:
+            raise RuntimeError(f"SceneIndex.regions: {total} hits exceed max_hits={max_hits}; raise the threshold or "
+                               f"max_hits")
+        off_host = (C.I64 * (S + 1))(*self._off)
+        parts = []
+        with torch.cuda.device(dev):
+            status = torch.zeros(1, dtype=torch.int32, device=dev)
+            for (q0, qs, ts), cnt, h in zip(slices, counts, totals):
+                m = qs.shape[0]
+                if qs.data_ptr() % 16:
+                    qs = qs.clone()
+                key = torch.empty(h, dtype=torch.int64, device=dev)
+                hsc = torch.empty(h, dtype=torch.float16, device=dev)
+                if h:
+                    ws_bytes = C.lib().osb_search_hits_workspace_bytes(S, m, h)
+                    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+                    C.call('osb_search_hits', C.ptr(self.rows), C.ptr(self.row_scene), self.n_rows, self.channels,
+                           off_host, S, C.ptr(qs), m, C.ptr(ts), C.ptr(cnt), h, C.ptr(key), C.ptr(hsc), C.ptr(status),
+                           C.ptr(ws), ws_bytes, C.stream_ptr())
+                    del ws
+                out = [torch.empty((m, R), dtype=torch.float16, device=dev)] + \
+                      [torch.empty((m, R), dtype=torch.int64, device=dev) for _ in range(3)] + \
+                      [torch.empty((m, R, 3), dtype=torch.int32, device=dev) for _ in range(2)] + \
+                      [torch.empty((S, m), dtype=torch.int64, device=dev)]
+                hit_out = [torch.empty(h, dtype=torch.int64, device=dev) for _ in range(4)] if hits else [None] * 4
+                ws_bytes = C.lib().osb_regions_workspace_bytes(h)
+                ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if h else None
+                C.call('osb_regions', C.ptr(key), C.ptr(hsc), h, C.ptr(self.coords), C.ptr(self.row_scene),
+                       C.ptr(self._off_dev), self.n_rows, S, m, R, int(reach), int(min_voxels), *[C.ptr(t) for t in out],
+                       *[C.ptr(t) for t in hit_out], C.ptr(status), C.ptr(ws), ws_bytes, C.stream_ptr())
+                del ws
+                if hits:
+                    hit_out[0] += q0
+                    parts.append(out + [hit_out[0], hit_out[1], hit_out[2], hsc, hit_out[3]])
+                else:
+                    parts.append(out + [None] * 5)
+            st = int(status.item())                                                         # host sync 2
+        if st & C_ST_RANGE:
+            raise RuntimeError("SceneIndex.regions: a hit's coordinate lies outside |x|, |y|, |z| < 2^17 - 256")
+        if st & C_ST_DUP:
+            raise RuntimeError("SceneIndex.regions: two hits of one (scene, query) share a voxel (duplicate coordinates)")
+        if st:
+            raise RuntimeError(f"SceneIndex.regions: the hit list does not match the search's counts (status {st})")
+        if len(parts) == 1:
+            return RegionResult(*parts[0])
+        cat = lambda j, d: None if parts[0][j] is None else torch.cat([p[j] for p in parts], dim=d)
+        return RegionResult(*[cat(j, 1 if j == 6 else 0) for j in range(12)])
+
     def _query(self, q, k, thr):
         nq, S, dev = q.shape[0], self.n_scenes, self.device
         if q.data_ptr() % 16:
@@ -146,6 +287,15 @@ class SceneIndex:
                    C.ptr(self._off_dev), S, C.ptr(q), nq, k, C.ptr(thr), C.ptr(score), C.ptr(scene), C.ptr(row),
                    C.ptr(smax), C.ptr(sarg), C.ptr(cnt), C.ptr(ws), ws_bytes, C.stream_ptr())
         return SearchResult(score, scene, row, smax, sarg, cnt)
+
+
+def regions_hit_bytes(n_hits, n_scenes, nq, hits=False):
+    """Device bytes a ``regions`` slice of nq queries holds at its peak for n_hits hits: the sorted hit list (10 B per
+    hit), the larger of the two workspaces, and the per-hit outputs (34 B per hit) when hits=True."""
+    if n_hits == 0:
+        return 0
+    ws = max(C.lib().osb_search_hits_workspace_bytes(n_scenes, nq, n_hits), C.lib().osb_regions_workspace_bytes(n_hits))
+    return 10 * n_hits + int(ws) + (32 * n_hits if hits else 0)
 
 
 def search_workspace_bytes(n_scenes, nq, k):
