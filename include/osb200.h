@@ -512,6 +512,27 @@ int osb_regions(const int64_t *hit_key, const void *hit_score_f16, int64_t n_hit
                 int32_t *box_min, int32_t *box_max, int64_t *n_regions, int64_t *hit_query, int64_t *hit_scene,
                 int64_t *hit_row, int64_t *hit_region, int32_t *status, void *ws, size_t ws_bytes, void *stream);
 
+/* FP8 scene index (DESIGN.md, "FP8 index contract"): each row stored as c e4m3 codes (uint8) and one int8 exponent e, the
+ * row it stands for being d = code * 2^e, an exact fp16 row.
+ *
+ * osb_index_quantize_f8: rows [n, c] (fp16 if rows_are_f16, else fp32, which is rounded to fp16 first) -> codes_out uint8
+ *   [n, c] and exp_out int8 [n].  e is the smallest integer with max|h| <= 448 * 2^e, clamped to [-15, 7]; codes are
+ *   e4m3(clamp(h * 2^-e, -448, 448)) rounded to nearest even; a row with a NaN or inf element gets NaN codes (0x7f) and
+ *   e = 0.  1 <= n < 2^31, rows and codes 16-byte aligned.  One launch, no host synchronisation.
+ * osb_search_f8 / osb_search_hits_f8: osb_search / osb_search_hits on the rows d, from codes [n_rows, c] (16-byte aligned)
+ *   and row_exp int8 [n_rows]; every output has the bits the fp16 entry point gives on d, with the same workspace. */
+int osb_index_quantize_f8(const void *rows, int32_t rows_are_f16, int64_t n, int32_t c, void *codes_out, int8_t *exp_out,
+                          void *stream);
+int osb_search_f8(const void *codes_f8, const int8_t *row_exp, const int32_t *row_scene, int64_t n_rows, int32_t c,
+                  const int64_t *scene_off_host, const int64_t *scene_off, int64_t n_scenes, const void *queries_f16,
+                  int32_t nq, int32_t k, const float *threshold, void *top_score_f16, int64_t *top_scene, int64_t *top_row,
+                  void *scene_max_f16, int64_t *scene_argmax, int64_t *scene_count, void *ws, size_t ws_bytes,
+                  void *stream);
+int osb_search_hits_f8(const void *codes_f8, const int8_t *row_exp, const int32_t *row_scene, int64_t n_rows, int32_t c,
+                       const int64_t *scene_off_host, int64_t n_scenes, const void *queries_f16, int32_t nq,
+                       const float *threshold, const int64_t *scene_count, int64_t n_hits, int64_t *hit_key,
+                       void *hit_score_f16, int32_t *status, void *ws, size_t ws_bytes, void *stream);
+
 /* Optional folded head (engine.forward_scores): rows z = [x L | x U] (fp32, row pitch ld floats) from one 1x1x1
  * convolution with the weights [L | U], W W^T = L L^T, U = W T^T  ->  score_k = fp16((x.U_k) / (|x L| + 1e-5)),
  * label = first argmax.  Same cosine scores as run/evaluate.py:305-310 without materialising the 768-d features. */

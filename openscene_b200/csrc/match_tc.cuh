@@ -1,10 +1,12 @@
 // The pieces of the tensor-core match (match_tc.cu) that the scene search (search.cu) multiplies with as well: the A
-// producers that load a 128-row tile and round it to the fp16 operand, the TMA stream of the 96-row text chunks, the
-// wgmma pass over one 96-column block, and the 64-bit order keys.  Whatever kernel calls them, a score is the same fp16
-// rounding of the same fp32 sum in the same order.  match_tc_body calls mt_fill_a; it keeps its TMA and wgmma loops written
-// out (the statements of mt_text_stage and mt_mma_pass), because calling the helpers there moves the register allocation of
-// some of its instantiations, and its kernels compile to the same instructions as before this header existed.
+// producers that load a 128-row tile and round it to the fp16 operand (mt_fill_a8: from the FP8 index's codes), the TMA
+// stream of the 96-row text chunks, the wgmma pass over one 96-column block, and the 64-bit order keys.  Whatever kernel
+// calls them, a score is the same fp16 rounding of the same fp32 sum in the same order.  match_tc_body calls mt_fill_a; it
+// keeps its TMA and wgmma loops written out (the statements of mt_text_stage and mt_mma_pass), because calling the helpers
+// there moves the register allocation of some of its instantiations, and its kernels compile to the same instructions as
+// before this header existed.
 #pragma once
+#include <cuda_fp8.h>
 #include "tc_ptx.cuh"
 
 namespace osb {
@@ -131,6 +133,57 @@ __device__ __forceinline__ void mt_fill_a(const MatchTcParams &p, uint8_t *sA, i
         asm volatile("st.shared.b32 [%0], %1;" ::"r"(line + j * (MT_M * 128)), "r"(*reinterpret_cast<const uint32_t *>(&h)) : "memory");
         if (p.feat_out != nullptr && live[u])
           reinterpret_cast<__half2 *>(p.feat_out)[pt * (C / 2) + lane + 32 * j] = h;
+      }
+    }
+  }
+}
+
+// FP8 A producer (warps 0..MT_PW-1; DESIGN.md, "FP8 index contract"): rows row0 .. row0 + 127 of e4m3 codes [n, C] and
+// their int8 exponents into the same K-major 128B-swizzled fp16 tile that mt_fill_a writes for the rows d = code * 2^e.
+// Every d is an fp16 number (the exponent rule keeps it in range, subnormals included), and both the unpack and the fp32
+// multiply by 2^e are exact, so the tile holds d bit for bit.  Rows at or past n are zero.  A lane loads 8 codes at once and
+// stores their 8 halves as one 16-byte swizzled unit.
+template <int NP>   // C = 64 * NP
+__device__ __forceinline__ void mt_fill_a8(const uint8_t *codes, const int8_t *row_exp, int64_t n, uint8_t *sA,
+                                           int64_t row0, int warp, int lane) {
+  constexpr int C = 64 * NP, U = NP / 4;          // C / 8 units of 8 codes per row, U per lane
+  constexpr int RB = 4, ROWS_PW = MT_M / MT_PW;    // 4 rows in flight per warp: as many bytes as mt_fill_a's 2 fp16 rows
+  for (int rr0 = 0; rr0 < ROWS_PW; rr0 += RB) {
+    uint2 v[RB][U];
+    int e[RB];
+#pragma unroll
+    for (int u = 0; u < RB; ++u) {
+      const int64_t pt = row0 + warp * ROWS_PW + rr0 + u;
+      if (pt < n) {
+        const uint2 *q = reinterpret_cast<const uint2 *>(codes + pt * C);
+#pragma unroll
+        for (int i = 0; i < U; ++i) v[u][i] = __ldg(q + lane + 32 * i);
+        e[u] = __ldg(row_exp + pt);
+      } else {
+#pragma unroll
+        for (int i = 0; i < U; ++i) v[u][i] = make_uint2(0u, 0u);
+        e[u] = 0;
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < RB; ++u) {
+      const int r = warp * ROWS_PW + rr0 + u;
+      const float sc = __int_as_float((127 + e[u]) << 23);                   // 2^e, e in [-15, 7]
+#pragma unroll
+      for (int i = 0; i < U; ++i) {
+        const int w = lane + 32 * i;   // elements 8w .. 8w + 7: depth chunk w / 8, 16-byte unit w % 8 of the 128-byte line
+        uint32_t h[4];
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          const uint32_t word = p < 2 ? v[u][i].x : v[u][i].y;
+          const __half2_raw raw = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(word >> (16 * (p & 1))), __NV_E4M3);
+          const float2 f = __half22float2(__half2(raw));
+          const __half2 d = __floats2half2_rn(f.x * sc, f.y * sc);
+          h[p] = *reinterpret_cast<const uint32_t *>(&d);
+        }
+        const uint32_t addr = smem_u32(sA) + (w >> 3) * (MT_M * 128) + r * 128 + (((w & 7) ^ (r & 7)) << 4);
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(h[0]), "r"(h[1]), "r"(h[2]), "r"(h[3])
+                     : "memory");
       }
     }
   }

@@ -46,6 +46,7 @@ struct SearchParams {
   uint64_t *hit_key;                       // [n_hits] (query << 32) | global row, in arrival order
   __half *hit_score;                       // [n_hits]
   int *status;                             // OSB_REGIONS_ST_COUNT when a segment's hits do not match its count
+  const int8_t *row_exp;                   // [n] FP8 storage (k_search<NP, HITS, true>): a.feat holds e4m3 codes [n, C]
 };
 
 __device__ __forceinline__ void scene_flush(const SearchParams &sp, int s, int q, uint64_t key, uint32_t cnt) {
@@ -76,8 +77,10 @@ __device__ __forceinline__ void hit_flush(const SearchParams &sp, const __half *
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // HITS = false: the search epilogue below.  HITS = true: the same loads, query stream and product; the epilogue writes
-// every (row, query) with float(s) >= thr[q] into the hit list instead (osb_search_hits).
-template <int NP, bool HITS = false>
+// every (row, query) with float(s) >= thr[q] into the hit list instead (osb_search_hits).  F8 = true: the rows are e4m3
+// codes with per-row exponents (osb_search_f8, osb_search_hits_f8); mt_fill_a8 writes the tile mt_fill_a writes for their
+// dequantized fp16 rows, and everything after the tile is the same.
+template <int NP, bool HITS = false, bool F8 = false>
 __global__ void __launch_bounds__(MT_THREADS, 1) k_search(const __grid_constant__ CUtensorMap tmQ, const SearchParams sp) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -115,15 +118,20 @@ __global__ void __launch_bounds__(MT_THREADS, 1) k_search(const __grid_constant_
     const int nrows = (int)std::min<int64_t>(MT_M, sp.n - row0);
     {   // the next tile's rows into L2 while this one is loaded, multiplied and scanned
       const int64_t nt = t + gridDim.x;
+      constexpr int ROW_BYTES = F8 ? C : 2 * C;
       if (nt < sp.n_tiles) {
-        const char *base = reinterpret_cast<const char *>(sp.a.feat) + nt * MT_M * (int64_t)(2 * C);
-        const int64_t bytes = std::min<int64_t>(MT_M, sp.n - nt * MT_M) * (2 * C);
+        const char *base = reinterpret_cast<const char *>(sp.a.feat) + nt * MT_M * (int64_t)ROW_BYTES;
+        const int64_t bytes = std::min<int64_t>(MT_M, sp.n - nt * MT_M) * ROW_BYTES;
         for (int64_t o = (int64_t)tid * 128; o < bytes; o += MT_PW * 32 * 128)
           asm volatile("prefetch.global.L2 [%0];" ::"l"(base + o));
+        if (F8 && tid == MT_PW * 32 - 1) asm volatile("prefetch.global.L2 [%0];" ::"l"(sp.row_exp + nt * MT_M));
       }
     }
     if (tid < MT_M) s_scene[tid] = tid < nrows ? __ldg(sp.row_scene + row0 + tid) : -1;
-    mt_fill_a<NP>(sp.a, sA, row0, warp, lane);
+    if constexpr (F8)
+      mt_fill_a8<NP>(reinterpret_cast<const uint8_t *>(sp.a.feat), sp.row_exp, sp.n, sA, row0, warp, lane);
+    else
+      mt_fill_a<NP>(sp.a, sA, row0, warp, lane);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic-proxy writes -> wgmma reads
     bar_sync(1, MT_PW * 32);
 
@@ -314,6 +322,81 @@ __global__ void k_hit_finish(const unsigned long long *__restrict__ cursor, cons
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_hits; i += stride) score_out[i] = score_in[slot[i]];
 }
 
+// FP8 index rows (DESIGN.md, "FP8 index contract"): one warp per row, 8 elements per lane and unit.  h = the row as fp16 (fp32
+// rows are rounded first), amax = max |h| by a warp reduction, e the smallest integer with amax <= 448 * 2^e clamped to
+// [-15, 7], codes = e4m3_rn(clamp(h * 2^-e, -448, 448)) by the hardware conversion; a row with a NaN or inf element gets NaN
+// codes (0x7f) and e = 0.  h * 2^-e is exact in fp32, so the conversion is the only rounding.
+template <int NP>
+__global__ void __launch_bounds__(256) k_index_quantize_f8(const void *__restrict__ rows, int rows_are_f16, int64_t n,
+                                                           uint8_t *__restrict__ codes, int8_t *__restrict__ row_exp) {
+  constexpr int C = 64 * NP, U = NP / 4;
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * 8;
+  for (int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n; r += warps) {
+    float v[U][8];
+    if (rows_are_f16) {
+      const uint4 *src = reinterpret_cast<const uint4 *>(rows) + r * (C / 8);
+#pragma unroll
+      for (int i = 0; i < U; ++i) {
+        const uint4 x = __ldg(src + lane + 32 * i);
+        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&w[p]));
+          v[i][2 * p] = f.x; v[i][2 * p + 1] = f.y;
+        }
+      }
+    } else {
+      const float4 *src = reinterpret_cast<const float4 *>(rows) + r * (C / 4);
+#pragma unroll
+      for (int i = 0; i < U; ++i) {
+        const float4 a = __ldg(src + 2 * (lane + 32 * i)), b = __ldg(src + 2 * (lane + 32 * i) + 1);
+        const float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[i][j] = __half2float(__float2half_rn(f[j]));      // the operand's `.half()`
+      }
+    }
+    float amax = 0.f;
+    bool bad = false;
+#pragma unroll
+    for (int i = 0; i < U; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        bad |= !isfinite(v[i][j]);
+        amax = fmaxf(amax, fabsf(v[i][j]));
+      }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    bad = __any_sync(0xffffffffu, bad);
+    int e = -15;
+    while (e < 7 && amax > 448.f * __int_as_float((127 + e) << 23)) ++e;
+    if (bad) e = 0;
+    const float sc = __int_as_float((127 - e) << 23);                                   // 2^-e
+    uint2 *dst = reinterpret_cast<uint2 *>(codes + r * C);
+#pragma unroll
+    for (int i = 0; i < U; ++i) {
+      uint32_t w[2];
+#pragma unroll
+      for (int p = 0; p < 2; ++p) {
+        uint32_t lo, hi;
+        {
+          const float2 x = make_float2(fminf(fmaxf(v[i][4 * p] * sc, -448.f), 448.f),
+                                       fminf(fmaxf(v[i][4 * p + 1] * sc, -448.f), 448.f));
+          lo = __nv_cvt_float2_to_fp8x2(x, __NV_SATFINITE, __NV_E4M3);
+        }
+        {
+          const float2 x = make_float2(fminf(fmaxf(v[i][4 * p + 2] * sc, -448.f), 448.f),
+                                       fminf(fmaxf(v[i][4 * p + 3] * sc, -448.f), 448.f));
+          hi = __nv_cvt_float2_to_fp8x2(x, __NV_SATFINITE, __NV_E4M3);
+        }
+        w[p] = bad ? 0x7f7f7f7fu : (lo | (hi << 16));
+      }
+      dst[lane + 32 * i] = make_uint2(w[0], w[1]);
+    }
+    if (lane == 0) row_exp[r] = (int8_t)e;
+  }
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -325,32 +408,37 @@ size_t osb_search_workspace_bytes(int64_t n_scenes, int32_t nq, int32_t k) {
   return (size_t)SR_MAX_GRID * nq * k * 8 + (size_t)2 * n_scenes * nq * 8;
 }
 
-int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
-               const int64_t *scene_off, int64_t n_scenes, const void *queries_f16, int32_t nq, int32_t k,
-               const float *threshold, void *top_score_f16, int64_t *top_scene, int64_t *top_row, void *scene_max_f16,
-               int64_t *scene_argmax, int64_t *scene_count, void *ws, size_t ws_bytes, void *stream_) {
+}  // extern "C"
+
+// osb_search (row_exp NULL: fp16 rows) and osb_search_f8 (e4m3 codes and their exponents); fn names the entry point in
+// the refusals
+static int search_run(const char *fn, const void *rows_f16, const int8_t *row_exp, const int32_t *row_scene,
+                      int64_t n_rows, int32_t c, const int64_t *scene_off_host, const int64_t *scene_off, int64_t n_scenes,
+                      const void *queries_f16, int32_t nq, int32_t k, const float *threshold, void *top_score_f16,
+                      int64_t *top_scene, int64_t *top_row, void *scene_max_f16, int64_t *scene_argmax,
+                      int64_t *scene_count, void *ws, size_t ws_bytes, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  OSB_CHECK(c == 512 || c == 768, "osb_search: feature width %d unsupported (OpenScene uses 512 / 768)", c);
-  OSB_CHECK(nq >= 1 && nq <= OSB_SEARCH_MAX_QUERIES, "osb_search: nq=%d outside 1..%d", nq, OSB_SEARCH_MAX_QUERIES);
-  OSB_CHECK(k >= 1 && k <= OSB_SEARCH_MAX_K, "osb_search: k=%d outside 1..%d", k, OSB_SEARCH_MAX_K);
-  OSB_CHECK(n_rows >= 1 && n_rows < (int64_t(1) << 31), "osb_search: N=%lld outside 1..2^31-1", (long long)n_rows);
-  OSB_CHECK(n_scenes >= 1 && n_scenes <= n_rows, "osb_search: %lld scenes for %lld rows", (long long)n_scenes,
+  OSB_CHECK(c == 512 || c == 768, "%s: feature width %d unsupported (OpenScene uses 512 / 768)", fn, c);
+  OSB_CHECK(nq >= 1 && nq <= OSB_SEARCH_MAX_QUERIES, "%s: nq=%d outside 1..%d", fn, nq, OSB_SEARCH_MAX_QUERIES);
+  OSB_CHECK(k >= 1 && k <= OSB_SEARCH_MAX_K, "%s: k=%d outside 1..%d", fn, k, OSB_SEARCH_MAX_K);
+  OSB_CHECK(n_rows >= 1 && n_rows < (int64_t(1) << 31), "%s: N=%lld outside 1..2^31-1", fn, (long long)n_rows);
+  OSB_CHECK(n_scenes >= 1 && n_scenes <= n_rows, "%s: %lld scenes for %lld rows", fn, (long long)n_scenes,
             (long long)n_rows);
   OSB_CHECK(rows_f16 && row_scene && scene_off_host && scene_off && queries_f16,
-            "osb_search: NULL rows, row scenes, scene offsets or queries");
+            "%s: NULL rows, row scenes, scene offsets or queries", fn);
   OSB_CHECK(top_score_f16 && top_scene && top_row && scene_max_f16 && scene_argmax,
-            "osb_search: NULL top-k or per-scene output");
-  OSB_CHECK(scene_count == nullptr || threshold != nullptr, "osb_search: scene counts need a threshold");
+            "%s: NULL top-k or per-scene output", fn);
+  OSB_CHECK(scene_count == nullptr || threshold != nullptr, "%s: scene counts need a threshold", fn);
   OSB_CHECK(((uintptr_t)rows_f16 & 15) == 0 && ((uintptr_t)queries_f16 & 15) == 0,
-            "osb_search: rows and queries must be 16-byte aligned");
+            "%s: rows and queries must be 16-byte aligned", fn);
   OSB_CHECK(scene_off_host[0] == 0 && scene_off_host[n_scenes] == n_rows,
-            "osb_search: scene offsets must run from 0 to N=%lld", (long long)n_rows);
+            "%s: scene offsets must run from 0 to N=%lld", fn, (long long)n_rows);
   for (int64_t s = 0; s < n_scenes; ++s)
-    OSB_CHECK(scene_off_host[s] < scene_off_host[s + 1], "osb_search: scene offsets not strictly increasing at scene %lld",
+    OSB_CHECK(scene_off_host[s] < scene_off_host[s + 1], "%s: scene offsets not strictly increasing at scene %lld", fn,
               (long long)s);
   const size_t need = osb_search_workspace_bytes(n_scenes, nq, k);
   OSB_CHECK(ws != nullptr && ws_bytes >= need && ((uintptr_t)ws & 7) == 0,
-            "osb_search: 8-byte aligned workspace of %zu bytes required (got %zu)", need, ws_bytes);
+            "%s: 8-byte aligned workspace of %zu bytes required (got %zu)", fn, need, ws_bytes);
 
   const int64_t n_tiles = ceil_div(n_rows, MT_M);
   int dev = 0, sms = SR_MAX_GRID;
@@ -360,7 +448,7 @@ int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, i
 
   SearchParams sp{};
   sp.a.feat = rows_f16; sp.a.feat_is_f16 = 1; sp.a.n_pts = n_rows; sp.a.C = c; sp.a.k_text = nq; sp.a.n_pass = 1;
-  sp.row_scene = row_scene; sp.n = n_rows; sp.n_tiles = n_tiles; sp.nq = nq; sp.k = k;
+  sp.row_scene = row_scene; sp.n = n_rows; sp.n_tiles = n_tiles; sp.nq = nq; sp.k = k; sp.row_exp = row_exp;
   sp.thr = scene_count ? threshold : nullptr;
   sp.lists = reinterpret_cast<uint64_t *>(ws);
   sp.scene_key = reinterpret_cast<unsigned long long *>(sp.lists + (size_t)SR_MAX_GRID * nq * k);
@@ -371,7 +459,13 @@ int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, i
   if (make_tmap_2b(&tmQ, queries_f16, (uint64_t)c, (uint64_t)nq, MT_NW, 1)) return 1;
   const int NP = c / 64;
   const size_t smem = (size_t)NP * MT_M * 128 + MT_BSTAGES * MT_NW * 128 + 128 + MT_M * 4 + 1024;
-  if (NP == 12) {
+  if (row_exp && NP == 12) {
+    OSB_SMEM_ATTR_ONCE((k_search<12, false, true>), 227 * 1024);
+    k_search<12, false, true><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  } else if (row_exp) {
+    OSB_SMEM_ATTR_ONCE((k_search<8, false, true>), 227 * 1024);
+    k_search<8, false, true><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  } else if (NP == 12) {
     OSB_SMEM_ATTR_ONCE(k_search<12>, 227 * 1024);
     k_search<12><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
   } else {
@@ -387,39 +481,65 @@ int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, i
   return 0;
 }
 
+extern "C" {
+
+int osb_search(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
+               const int64_t *scene_off, int64_t n_scenes, const void *queries_f16, int32_t nq, int32_t k,
+               const float *threshold, void *top_score_f16, int64_t *top_scene, int64_t *top_row, void *scene_max_f16,
+               int64_t *scene_argmax, int64_t *scene_count, void *ws, size_t ws_bytes, void *stream) {
+  return search_run("osb_search", rows_f16, nullptr, row_scene, n_rows, c, scene_off_host, scene_off, n_scenes,
+                    queries_f16, nq, k, threshold, top_score_f16, top_scene, top_row, scene_max_f16, scene_argmax,
+                    scene_count, ws, ws_bytes, stream);
+}
+
+int osb_search_f8(const void *codes_f8, const int8_t *row_exp, const int32_t *row_scene, int64_t n_rows, int32_t c,
+                  const int64_t *scene_off_host, const int64_t *scene_off, int64_t n_scenes, const void *queries_f16,
+                  int32_t nq, int32_t k, const float *threshold, void *top_score_f16, int64_t *top_scene, int64_t *top_row,
+                  void *scene_max_f16, int64_t *scene_argmax, int64_t *scene_count, void *ws, size_t ws_bytes,
+                  void *stream) {
+  OSB_CHECK(row_exp != nullptr, "osb_search_f8: NULL row exponents");
+  return search_run("osb_search_f8", codes_f8, row_exp, row_scene, n_rows, c, scene_off_host, scene_off, n_scenes,
+                    queries_f16, nq, k, threshold, top_score_f16, top_scene, top_row, scene_max_f16, scene_argmax,
+                    scene_count, ws, ws_bytes, stream);
+}
+
 size_t osb_search_hits_workspace_bytes(int64_t n_scenes, int32_t nq, int64_t n_hits) {
   if (n_scenes < 1 || nq < 1 || nq > OSB_SEARCH_MAX_QUERIES || n_hits < 1 || n_hits >= (int64_t(1) << 31)) return 0;
   // arrival keys 8, two payloads 4 + 4, arrival scores 2 (rounded up to 8 B per 4 hits), two [nq][S] arrays, sort histogram
   return (size_t)n_hits * 16 + (size_t)((n_hits + 3) / 4) * 8 + (size_t)2 * n_scenes * nq * 8 + radix_sort_ws_bytes(n_hits);
 }
 
-int osb_search_hits(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
-                    int64_t n_scenes, const void *queries_f16, int32_t nq, const float *threshold,
-                    const int64_t *scene_count, int64_t n_hits, int64_t *hit_key, void *hit_score_f16, int32_t *status,
-                    void *ws, size_t ws_bytes, void *stream_) {
+}  // extern "C"
+
+// osb_search_hits (row_exp NULL: fp16 rows) and osb_search_hits_f8 (e4m3 codes and their exponents)
+static int search_hits_run(const char *fn, const void *rows_f16, const int8_t *row_exp, const int32_t *row_scene,
+                           int64_t n_rows, int32_t c, const int64_t *scene_off_host, int64_t n_scenes,
+                           const void *queries_f16, int32_t nq, const float *threshold, const int64_t *scene_count,
+                           int64_t n_hits, int64_t *hit_key, void *hit_score_f16, int32_t *status, void *ws,
+                           size_t ws_bytes, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  OSB_CHECK(c == 512 || c == 768, "osb_search_hits: feature width %d unsupported (OpenScene uses 512 / 768)", c);
-  OSB_CHECK(nq >= 1 && nq <= OSB_SEARCH_MAX_QUERIES, "osb_search_hits: nq=%d outside 1..%d", nq, OSB_SEARCH_MAX_QUERIES);
-  OSB_CHECK(n_rows >= 1 && n_rows < (int64_t(1) << 31), "osb_search_hits: N=%lld outside 1..2^31-1", (long long)n_rows);
-  OSB_CHECK(n_scenes >= 1 && n_scenes <= n_rows, "osb_search_hits: %lld scenes for %lld rows", (long long)n_scenes,
+  OSB_CHECK(c == 512 || c == 768, "%s: feature width %d unsupported (OpenScene uses 512 / 768)", fn, c);
+  OSB_CHECK(nq >= 1 && nq <= OSB_SEARCH_MAX_QUERIES, "%s: nq=%d outside 1..%d", fn, nq, OSB_SEARCH_MAX_QUERIES);
+  OSB_CHECK(n_rows >= 1 && n_rows < (int64_t(1) << 31), "%s: N=%lld outside 1..2^31-1", fn, (long long)n_rows);
+  OSB_CHECK(n_scenes >= 1 && n_scenes <= n_rows, "%s: %lld scenes for %lld rows", fn, (long long)n_scenes,
             (long long)n_rows);
-  OSB_CHECK(n_hits >= 1 && n_hits < (int64_t(1) << 31), "osb_search_hits: n_hits=%lld outside 1..2^31-1",
+  OSB_CHECK(n_hits >= 1 && n_hits < (int64_t(1) << 31), "%s: n_hits=%lld outside 1..2^31-1", fn,
             (long long)n_hits);
   OSB_CHECK(rows_f16 && row_scene && scene_off_host && queries_f16 && threshold && scene_count,
-            "osb_search_hits: NULL rows, row scenes, scene offsets, queries, threshold or scene counts");
-  OSB_CHECK(hit_key && hit_score_f16 && status, "osb_search_hits: NULL hit list or status");
+            "%s: NULL rows, row scenes, scene offsets, queries, threshold or scene counts", fn);
+  OSB_CHECK(hit_key && hit_score_f16 && status, "%s: NULL hit list or status", fn);
   OSB_CHECK(((uintptr_t)rows_f16 & 15) == 0 && ((uintptr_t)queries_f16 & 15) == 0,
-            "osb_search_hits: rows and queries must be 16-byte aligned");
+            "%s: rows and queries must be 16-byte aligned", fn);
   OSB_CHECK(((uintptr_t)hit_key & 7) == 0 && ((uintptr_t)hit_score_f16 & 1) == 0 && ((uintptr_t)status & 3) == 0,
-            "osb_search_hits: misaligned hit list or status");
+            "%s: misaligned hit list or status", fn);
   OSB_CHECK(scene_off_host[0] == 0 && scene_off_host[n_scenes] == n_rows,
-            "osb_search_hits: scene offsets must run from 0 to N=%lld", (long long)n_rows);
+            "%s: scene offsets must run from 0 to N=%lld", fn, (long long)n_rows);
   for (int64_t s = 0; s < n_scenes; ++s)
     OSB_CHECK(scene_off_host[s] < scene_off_host[s + 1],
-              "osb_search_hits: scene offsets not strictly increasing at scene %lld", (long long)s);
+              "%s: scene offsets not strictly increasing at scene %lld", fn, (long long)s);
   const size_t need = osb_search_hits_workspace_bytes(n_scenes, nq, n_hits);
   OSB_CHECK(ws != nullptr && ws_bytes >= need && ((uintptr_t)ws & 7) == 0,
-            "osb_search_hits: 8-byte aligned workspace of %zu bytes required (got %zu)", need, ws_bytes);
+            "%s: 8-byte aligned workspace of %zu bytes required (got %zu)", fn, need, ws_bytes);
 
   uint8_t *w = reinterpret_cast<uint8_t *>(ws);
   uint64_t *keys_a = reinterpret_cast<uint64_t *>(w);                       w += (size_t)n_hits * 8;
@@ -441,14 +561,20 @@ int osb_search_hits(const void *rows_f16, const int32_t *row_scene, int64_t n_ro
   SearchParams sp{};
   sp.a.feat = rows_f16; sp.a.feat_is_f16 = 1; sp.a.n_pts = n_rows; sp.a.C = c; sp.a.k_text = nq; sp.a.n_pass = 1;
   sp.row_scene = row_scene; sp.n = n_rows; sp.n_tiles = n_tiles; sp.nq = nq; sp.k = 1;
-  sp.thr = threshold;
+  sp.thr = threshold; sp.row_exp = row_exp;
   sp.n_scenes = n_scenes; sp.cursor = cursor; sp.seg_end = seg_end; sp.hit_key = keys_a; sp.hit_score = score_a;
   sp.status = status;
   CUtensorMap tmQ;
   if (make_tmap_2b(&tmQ, queries_f16, (uint64_t)c, (uint64_t)nq, MT_NW, 1)) return 1;
   const int NP = c / 64;
   const size_t smem = (size_t)NP * MT_M * 128 + MT_BSTAGES * MT_NW * 128 + 128 + MT_M * 4 + 1024;
-  if (NP == 12) {
+  if (row_exp && NP == 12) {
+    OSB_SMEM_ATTR_ONCE((k_search<12, true, true>), 227 * 1024);
+    k_search<12, true, true><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  } else if (row_exp) {
+    OSB_SMEM_ATTR_ONCE((k_search<8, true, true>), 227 * 1024);
+    k_search<8, true, true><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
+  } else if (NP == 12) {
     OSB_SMEM_ATTR_ONCE((k_search<12, true>), 227 * 1024);
     k_search<12, true><<<grid, MT_THREADS, smem, stream>>>(tmQ, sp);
   } else {
@@ -460,12 +586,50 @@ int osb_search_hits(const void *rows_f16, const int32_t *row_scene, int64_t n_ro
   // canonical order: stable sort by (query << 32) | global row, distinct per hit (bits 0..38: q < 96, row < 2^31)
   uint64_t *keys_out = reinterpret_cast<uint64_t *>(hit_key);
   const int where = radix_sort_pairs(keys_a, vals_a, keys_out, vals_b, nullptr, n_hits, 0, 39, sort_ws, stream);
-  OSB_CHECK(where >= 0, "osb_search_hits: sort launch failed");
+  OSB_CHECK(where >= 0, "%s: sort launch failed", fn);
   const int32_t *slot = where ? vals_b : vals_a;
   if (where == 0) OSB_CUDA(cudaMemcpyAsync(keys_out, keys_a, (size_t)n_hits * 8, cudaMemcpyDeviceToDevice, stream));
   const int blocks = (int)std::min<int64_t>(ceil_div(std::max<int64_t>(n_hits, n_scenes * nq), 256), 4096);
   k_hit_finish<<<blocks, 256, 0, stream>>>(cursor, seg_end, n_scenes * nq, slot, score_a, n_hits,
                                            (__half *)hit_score_f16, status);
+  OSB_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" {
+
+int osb_search_hits(const void *rows_f16, const int32_t *row_scene, int64_t n_rows, int32_t c, const int64_t *scene_off_host,
+                    int64_t n_scenes, const void *queries_f16, int32_t nq, const float *threshold,
+                    const int64_t *scene_count, int64_t n_hits, int64_t *hit_key, void *hit_score_f16, int32_t *status,
+                    void *ws, size_t ws_bytes, void *stream) {
+  return search_hits_run("osb_search_hits", rows_f16, nullptr, row_scene, n_rows, c, scene_off_host, n_scenes, queries_f16,
+                         nq, threshold, scene_count, n_hits, hit_key, hit_score_f16, status, ws, ws_bytes, stream);
+}
+
+int osb_search_hits_f8(const void *codes_f8, const int8_t *row_exp, const int32_t *row_scene, int64_t n_rows, int32_t c,
+                       const int64_t *scene_off_host, int64_t n_scenes, const void *queries_f16, int32_t nq,
+                       const float *threshold, const int64_t *scene_count, int64_t n_hits, int64_t *hit_key,
+                       void *hit_score_f16, int32_t *status, void *ws, size_t ws_bytes, void *stream) {
+  OSB_CHECK(row_exp != nullptr, "osb_search_hits_f8: NULL row exponents");
+  return search_hits_run("osb_search_hits_f8", codes_f8, row_exp, row_scene, n_rows, c, scene_off_host, n_scenes,
+                         queries_f16, nq, threshold, scene_count, n_hits, hit_key, hit_score_f16, status, ws, ws_bytes,
+                         stream);
+}
+
+int osb_index_quantize_f8(const void *rows, int32_t rows_are_f16, int64_t n, int32_t c, void *codes_out, int8_t *exp_out,
+                          void *stream) {
+  OSB_CHECK(c == 512 || c == 768, "osb_index_quantize_f8: feature width %d unsupported (OpenScene uses 512 / 768)", c);
+  OSB_CHECK(n >= 1 && n < (int64_t(1) << 31), "osb_index_quantize_f8: N=%lld outside 1..2^31-1", (long long)n);
+  OSB_CHECK(rows && codes_out && exp_out, "osb_index_quantize_f8: NULL rows, codes or exponents");
+  OSB_CHECK(((uintptr_t)rows & 15) == 0 && ((uintptr_t)codes_out & 15) == 0,
+            "osb_index_quantize_f8: rows and codes must be 16-byte aligned");
+  const int blocks = (int)std::min<int64_t>(ceil_div(n, 8), 132 * 16);
+  if (c == 768)
+    k_index_quantize_f8<12><<<blocks, 256, 0, (cudaStream_t)stream>>>(rows, rows_are_f16 != 0, n,
+                                                                       (uint8_t *)codes_out, exp_out);
+  else
+    k_index_quantize_f8<8><<<blocks, 256, 0, (cudaStream_t)stream>>>(rows, rows_are_f16 != 0, n, (uint8_t *)codes_out,
+                                                                      exp_out);
   OSB_LAUNCH_CHECK();
   return 0;
 }

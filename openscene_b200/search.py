@@ -14,6 +14,10 @@ the index once; more queries run slice after slice.  Nothing synchronises the ho
 An index built with ``coords=True`` also keeps each row's voxel coordinates, and ``regions`` groups each query's hits
 (rows at or above a threshold) into spatially connected regions on the device (csrc/regions.cu; DESIGN.md, "Region
 contract"): the objects a search for a name or an image is after, with their boxes, sizes and best hits.
+
+An index built with ``storage='fp8'`` keeps each row as e4m3 codes and one power-of-two exponent (C + 1 bytes instead of
+2 C; DESIGN.md, "FP8 index contract"): twice the rows in the same memory, and each query slice reads half the bytes.  It
+answers exactly what an fp16 index holding the dequantized rows answers.
 """
 from collections import namedtuple
 
@@ -44,9 +48,15 @@ class SceneIndex:
     """A fixed device arena of fp16 operand rows [capacity_rows, channels], filled scene after scene by ``add``.
 
     Scene ids follow the order of ``add``.  The arena never grows and is never re-copied.  With ``coords=True`` an int32
-    [capacity_rows, 4] arena holds each row's voxel coordinates (x, y, z, 0), which ``regions`` needs."""
+    [capacity_rows, 4] arena holds each row's voxel coordinates (x, y, z, 0), which ``regions`` needs.
 
-    def __init__(self, capacity_rows, channels=768, device=None, coords=False):
+    ``storage='fp8'`` stores each row as e4m3 codes (``codes``, uint8 [capacity_rows, channels]) and an int8 exponent
+    (``row_exp``, [capacity_rows]) instead of ``rows``: the row it stands for is d = code * 2^e, an exact fp16 row, and
+    every result is the one an fp16 index holding d gives.  C + 5 bytes per row with the scene id, against 2 C + 4."""
+
+    def __init__(self, capacity_rows, channels=768, device=None, coords=False, storage='fp16'):
+        if storage not in ('fp16', 'fp8'):
+            raise ValueError(f"SceneIndex: storage must be 'fp16' or 'fp8' (got {storage!r})")
         if channels not in (512, 768):
             raise ValueError(f"SceneIndex: channels must be 512 or 768 (got {channels})")
         if not 1 <= capacity_rows < 2 ** 31:
@@ -58,7 +68,14 @@ class SceneIndex:
             self.device = torch.device('cuda', torch.cuda.current_device())
         self.capacity = int(capacity_rows)
         self.channels = int(channels)
-        self.rows = torch.empty((self.capacity, self.channels), dtype=torch.float16, device=self.device)
+        self.storage = storage
+        if storage == 'fp16':
+            self.rows = torch.empty((self.capacity, self.channels), dtype=torch.float16, device=self.device)
+            self.codes = self.row_exp = None
+        else:
+            self.rows = None
+            self.codes = torch.empty((self.capacity, self.channels), dtype=torch.uint8, device=self.device)
+            self.row_exp = torch.empty(self.capacity, dtype=torch.int8, device=self.device)
         self.row_scene = torch.empty(self.capacity, dtype=torch.int32, device=self.device)
         self.coords = torch.zeros((self.capacity, 4), dtype=torch.int32, device=self.device) if coords else None
         self._off = [0]                                    # host offsets, n_scenes + 1
@@ -74,8 +91,19 @@ class SceneIndex:
         return len(self._off) - 1
 
     def scene_rows(self, scene):
-        """The rows [n, C] of one scene (a view into the arena)."""
-        return self.rows[self._off[scene]:self._off[scene + 1]]
+        """The rows [n, C] of one scene: a view into the arena, or on an FP8 index a new fp16 tensor of the dequantized
+        rows d = code * 2^e (exact; NaN rows stay NaN)."""
+        a, b = self._off[scene], self._off[scene + 1]
+        if self.codes is None:
+            return self.rows[a:b]
+        scale = ((self.row_exp[a:b].int() + 127) << 23).view(torch.float32)       # 2^e, exactly
+        return (self.codes[a:b].view(torch.float8_e4m3fn).float() * scale[:, None]).half()
+
+    def _operand(self):
+        """the entry-point suffix and the row arguments of the storage"""
+        if self.codes is None:
+            return '', [C.ptr(self.rows)]
+        return '_f8', [C.ptr(self.codes), C.ptr(self.row_exp)]
 
     def scene_coords(self, scene):
         """The voxel coordinates [n, 4] (x, y, z, 0) of one scene, row for row with ``scene_rows`` (a view)."""
@@ -88,7 +116,7 @@ class SceneIndex:
         its scene id.  ``coords``: integer voxel coordinates [n, 3], or [n, 4] in MinkowskiEngine's (batch, x, y, z)
         layout whose batch column is dropped, row for row with ``rows``; required on an index built with coordinates and
         refused on one without.  An empty scene, a wrong width, dtype or device, or a full arena is refused before
-        anything is copied."""
+        anything is copied.  An FP8 index quantizes the rows on the device (``osb_index_quantize_f8``, one launch)."""
         if not isinstance(rows, torch.Tensor) or rows.dim() != 2:
             raise ValueError("SceneIndex.add: rows must be a 2-D tensor [n, C]")
         if rows.dtype not in (torch.float16, torch.float32):
@@ -117,7 +145,15 @@ class SceneIndex:
         if o + n > self.capacity:
             raise RuntimeError(f"SceneIndex.add: {n} rows do not fit ({self.capacity - o} of {self.capacity} left)")
         s = self.n_scenes
-        self.rows[o:o + n].copy_(rows)                    # fp32 -> fp16 rounds to nearest even, as `.half()`
+        if self.codes is None:
+            self.rows[o:o + n].copy_(rows)                # fp32 -> fp16 rounds to nearest even, as `.half()`
+        else:
+            src = rows.contiguous()
+            if src.data_ptr() % 16:
+                src = src.clone()
+            with torch.cuda.device(self.device):
+                C.call('osb_index_quantize_f8', C.ptr(src), int(src.dtype == torch.float16), n, self.channels,
+                       C.ptr(self.codes[o:o + n]), C.ptr(self.row_exp[o:o + n]), C.stream_ptr())
         self.row_scene[o:o + n].fill_(s)
         if self.coords is not None:
             self.coords[o:o + n, :3].copy_(coords[:, -3:])
@@ -125,7 +161,7 @@ class SceneIndex:
             grown = torch.zeros(2 * self._off_dev.numel(), dtype=torch.int64, device=self.device)
             grown[:self._off_dev.numel()].copy_(self._off_dev)
             self._off_dev = grown
-        self._off_dev[s + 1] = o + n
+        self._off_dev[s + 1:s + 2].fill_(o + n)           # a fill kernel, not a copy from host memory
         self._off.append(o + n)
         self.names.append(name)
         return s
@@ -237,7 +273,8 @@ class SceneIndex:
                 if h:
                     ws_bytes = C.lib().osb_search_hits_workspace_bytes(S, m, h)
                     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-                    C.call('osb_search_hits', C.ptr(self.rows), C.ptr(self.row_scene), self.n_rows, self.channels,
+                    sfx, operand = self._operand()
+                    C.call('osb_search_hits' + sfx, *operand, C.ptr(self.row_scene), self.n_rows, self.channels,
                            off_host, S, C.ptr(qs), m, C.ptr(ts), C.ptr(cnt), h, C.ptr(key), C.ptr(hsc), C.ptr(status),
                            C.ptr(ws), ws_bytes, C.stream_ptr())
                     del ws
@@ -283,7 +320,8 @@ class SceneIndex:
             ws_bytes = C.lib().osb_search_workspace_bytes(S, nq, k)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
             off_host = (C.I64 * (S + 1))(*self._off)
-            C.call('osb_search', C.ptr(self.rows), C.ptr(self.row_scene), self.n_rows, self.channels, off_host,
+            sfx, operand = self._operand()
+            C.call('osb_search' + sfx, *operand, C.ptr(self.row_scene), self.n_rows, self.channels, off_host,
                    C.ptr(self._off_dev), S, C.ptr(q), nq, k, C.ptr(thr), C.ptr(score), C.ptr(scene), C.ptr(row),
                    C.ptr(smax), C.ptr(sarg), C.ptr(cnt), C.ptr(ws), ws_bytes, C.stream_ptr())
         return SearchResult(score, scene, row, smax, sarg, cnt)
