@@ -533,6 +533,35 @@ int osb_search_hits_f8(const void *codes_f8, const int8_t *row_exp, const int32_
                        const float *threshold, const int64_t *scene_count, int64_t n_hits, int64_t *hit_key,
                        void *hit_score_f16, int32_t *status, void *ws, size_t ws_bytes, void *stream);
 
+/* Sharded scene index (DESIGN.md, "Sharded index contract"): the per-rank results of osb_search / osb_regions merged into
+ * the results of one index holding every scene in ascending global id.  The directory maps each rank's local scene to its
+ * global id (scene_gid int64 [n_local]) and each global id to its first global row (row_base int64 [n_global]).
+ *
+ * osb_shard_keys: a rank's decoded results score_f16 fp16 / scene int64 (local, -1 padding) / row int64 [n] -> key int64
+ *   [n]: bits 48-63 the score's order (as osb_search's key: -0 == +0, inf above every finite value), bits 0-47 ~(row_base[g]
+ *   + row), 0 for NaN and padding; global_scene int64 [n]: g = scene_gid[scene], -1 for padding.  Refused when the group
+ *   holds 2^48 rows or more (n_rows_global).
+ * osb_shard_merge: keys int64 [world][nq][m], each [nq][m] list in descending key order -> winners int64 [nq][m]: the
+ *   source position w * m + j of the m largest keys per query, largest first (ties among 0 keys to the lower w * m + j).
+ *   1 <= world <= OSB_SHARD_MAX_WORLD, 1 <= nq <= OSB_SHARD_MAX_QUERIES, 1 <= m <= OSB_SHARD_MAX_M.
+ * osb_shard_hits: the gathered hit lists of one query slice, hit_query (< nq) / hit_grow (global row) / hit_rank (source
+ *   rank) / hit_region (rank in the source rank's list, or -1) int64 [n_hits], and the winners int64 [nq][R] of the region
+ *   merge -> order int64 [n_hits]: the hits sorted by (query, global row) (a stable radix sort), as source positions;
+ *   region_out int64 [n_hits]: per sorted hit the rank of its region in the merged list, -1 when the region is not in it.
+ *   The workspace (osb_shard_hits_workspace_bytes, 256-byte aligned) is overwritten.
+ * Pointers 8-byte aligned (scores 2).  Integer work only; no host synchronisation. */
+#define OSB_SHARD_MAX_WORLD 64
+#define OSB_SHARD_MAX_QUERIES 65535
+#define OSB_SHARD_MAX_M 32
+int osb_shard_keys(const void *score_f16, const int64_t *scene, const int64_t *row, int64_t n, const int64_t *scene_gid,
+                   int64_t n_local, const int64_t *row_base, int64_t n_global, int64_t n_rows_global, int64_t *key,
+                   int64_t *global_scene, void *stream);
+int osb_shard_merge(const int64_t *keys, int32_t world, int32_t nq, int32_t m, int64_t *winners, void *stream);
+size_t osb_shard_hits_workspace_bytes(int64_t n_hits);
+int osb_shard_hits(const int64_t *hit_query, const int64_t *hit_grow, const int64_t *hit_rank, const int64_t *hit_region,
+                   int64_t n_hits, int32_t world, int32_t nq, int32_t R, const int64_t *winners, int64_t *order,
+                   int64_t *region_out, void *ws, size_t ws_bytes, void *stream);
+
 /* Optional folded head (engine.forward_scores): rows z = [x L | x U] (fp32, row pitch ld floats) from one 1x1x1
  * convolution with the weights [L | U], W W^T = L L^T, U = W T^T  ->  score_k = fp16((x.U_k) / (|x L| + 1e-5)),
  * label = first argmax.  Same cosine scores as run/evaluate.py:305-310 without materialising the 768-d features. */

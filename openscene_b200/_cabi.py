@@ -85,6 +85,10 @@ SIGNATURES = {
     'osb_index_quantize_f8': (c_int, [P, I32, I64, I32, P, P, P]),
     'osb_search_f8': (c_int, [P, P, P, I64, I32, P, P, I64, P, I32, I32, P, P, P, P, P, P, P, P, SZ, P]),
     'osb_search_hits_f8': (c_int, [P, P, P, I64, I32, P, I64, P, I32, P, P, I64, P, P, P, P, SZ, P]),
+    'osb_shard_keys': (c_int, [P, P, P, I64, P, I64, P, I64, I64, P, P, P]),
+    'osb_shard_merge': (c_int, [P, I32, I32, I32, P, P]),
+    'osb_shard_hits_workspace_bytes': (SZ, [I64]),
+    'osb_shard_hits': (c_int, [P, P, P, P, I64, I32, I32, I32, P, P, P, P, SZ, P]),
     'osb_folded_head_finish': (c_int, [P, I64, I32, I32, I32, P, P, P, P]),
     'osb_voxelize_workspace_bytes': (SZ, [I64]),
     'osb_voxelize': (c_int, [P, I32, I64, POINTER(c_double), P, P, P, POINTER(I64), POINTER(c_double), P, SZ, P]),

@@ -18,7 +18,14 @@ contract"): the objects a search for a name or an image is after, with their box
 An index built with ``storage='fp8'`` keeps each row as e4m3 codes and one power-of-two exponent (C + 1 bytes instead of
 2 C; DESIGN.md, "FP8 index contract"): twice the rows in the same memory, and each query slice reads half the bytes.  It
 answers exactly what an fp16 index holding the dequantized rows answers.
+
+``ShardedSceneIndex`` spreads one database over the ranks of a process group (csrc/shard.cu; DESIGN.md, "Sharded index
+contract"): each rank keeps the scenes it computed, a query runs ``k_search`` on every shard, and the small per-shard
+results are merged on the device after one collective.  Every output is bit for bit the output of one ``SceneIndex``
+that adds the scenes in ascending global id.
 """
+import bisect
+import operator
 from collections import namedtuple
 
 import torch
@@ -325,6 +332,410 @@ class SceneIndex:
                    C.ptr(self._off_dev), S, C.ptr(q), nq, k, C.ptr(thr), C.ptr(score), C.ptr(scene), C.ptr(row),
                    C.ptr(smax), C.ptr(sarg), C.ptr(cnt), C.ptr(ws), ws_bytes, C.stream_ptr())
         return SearchResult(score, scene, row, smax, sarg, cnt)
+
+
+MAX_WORLD = 64        # OSB_SHARD_MAX_WORLD
+MAX_SHARD_QUERIES = 65535    # OSB_SHARD_MAX_QUERIES
+
+Directory = namedtuple('Directory', 'owner local rows base n_local names')
+Directory.__doc__ = """Per global scene id: owner rank, local scene on that rank, row count, first global row (lists of
+length S); n_local: scenes per rank; names: per global id."""
+
+
+def build_directory(ids, rows, names, channels, storage, group=None):
+    """The directory of a sharded index, built collectively: one ``all_gather_object`` of every rank's (global ids, row
+    counts, names, width, storage), checked alike on every rank, so that a refusal is the same ValueError everywhere.
+    The ids over the group must be exactly 0 .. S-1, the widths and storages equal.  No device work: this runs over any
+    backend and without a GPU."""
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    mine = ([int(i) for i in ids], [int(r) for r in rows], list(names), int(channels), str(storage))
+    every = [None] * world
+    dist.all_gather_object(every, mine, group=group)
+    for what, j in (('widths', 3), ('storages', 4)):
+        vals = [e[j] for e in every]
+        if len(set(vals)) > 1:
+            raise ValueError(f"ShardedSceneIndex: the {what} differ over the group (per rank: {vals})")
+    S = sum(len(e[0]) for e in every)
+    owner, local, count = [None] * S, [None] * S, [None] * S
+    out_of_range = []
+    for w, (ids_w, rows_w, _, _, _) in enumerate(every):
+        for j, (g, n) in enumerate(zip(ids_w, rows_w)):
+            if not 0 <= g < S:
+                out_of_range.append(g)
+                continue
+            if owner[g] is not None:
+                raise ValueError(f"ShardedSceneIndex: scene id {g} is held twice (ranks {owner[g]} and {w})")
+            owner[g], local[g], count[g] = w, j, n
+    if out_of_range:
+        missing = [g for g in range(S) if owner[g] is None]
+        raise ValueError(f"ShardedSceneIndex: the scene ids over the group must be 0 .. {S - 1}; id {missing[0]} is "
+                         f"missing (ids outside the range: {sorted(out_of_range)[:8]})")
+    base, run = [], 0
+    for n in count:
+        base.append(run)
+        run += n
+    if run >= 2 ** 48:
+        raise ValueError(f"ShardedSceneIndex: {run} rows over the group; the merge keys hold global rows below 2^48")
+    gnames = [every[owner[g]][2][local[g]] for g in range(S)]
+    return Directory(owner, local, count, base, [len(e[0]) for e in every], gnames)
+
+
+def _rotate(t, a, o, e):
+    """Move rows t[o:e] to t[a:a + e - o] and rows t[a:o] up behind them, on the device: the tail is copied aside, and
+    the rows in between move in chunks from the top down through a bounce buffer (copies of overlapping memory are not
+    allowed), at most 2^16 rows at a time."""
+    n = e - o
+    if o == a:
+        return
+    tail = t[o:e].clone()
+    step = max(n, 1 << 16)
+    buf = None if step == n else torch.empty((min(step, o - a),) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+    hi = o
+    while hi > a:
+        lo = max(a, hi - step)
+        if buf is None:
+            t[lo + n:hi + n].copy_(t[lo:hi])              # n rows apart, at most n rows long: no overlap
+        else:
+            b = buf[:hi - lo]
+            b.copy_(t[lo:hi])
+            t[lo + n:hi + n].copy_(b)
+        hi = lo
+    t[a:a + n].copy_(tail)
+
+
+class ShardedSceneIndex:
+    """One database of scenes spread over the ranks of a process group (``process_group=None``: the default group).
+
+    Each rank owns a ``SceneIndex`` (``local``) of the given capacity, width, storage and coordinates, and holds the
+    scenes it added.  ``add`` is local and takes the scene's global id.  ``query``, ``regions`` and ``sync`` are
+    collectives: every rank calls them in the same order with the same arguments.  Their outputs are, on every rank,
+    bit for bit those of one ``SceneIndex`` that adds every scene in ascending global id, whatever the assignment of
+    scenes to ranks and the order of the local adds.
+
+    The directory (global id -> owner rank, local scene, row count, first global row) is built by ``sync``: one
+    ``all_gather_object`` and one host synchronisation per change of the index.  ``query`` and ``regions`` call it on a
+    rank that has added since the last build (or never built it), which covers the usual case of every rank adding its
+    share before the first query.  A rank cannot learn of another rank's add without a host round trip, which ``query``
+    does not make: after adds on some ranks only, call ``sync()`` on every rank.
+
+    A rank keeps its scenes in ascending global id, so that its local row order is the global row order: ties inside
+    a rank's top-k then fall as they fall in the single index.  An ``add`` out of that order moves the rows of the
+    rank's scenes with higher ids up on the device (cost proportional to them; ``DistributedSampler`` with
+    ``shuffle=False`` never does it)."""
+
+    def __init__(self, capacity_rows, channels=768, process_group=None, device=None, coords=False, storage='fp16'):
+        import torch.distributed as dist
+        if not dist.is_available() or not dist.is_initialized():
+            raise RuntimeError("ShardedSceneIndex: torch.distributed is not initialised")
+        self.group = process_group if process_group is not None else dist.group.WORLD
+        self.rank, self.world = dist.get_rank(self.group), dist.get_world_size(self.group)
+        if self.world > MAX_WORLD:
+            raise ValueError(f"ShardedSceneIndex: {self.world} ranks; at most {MAX_WORLD}")
+        self.local = SceneIndex(capacity_rows, channels, device=device, coords=coords, storage=storage)
+        self.device = self.local.device
+        self._ids = []              # global id of each local scene, ascending (= the local scene order)
+        self._dir = None
+
+    # ------------------------------------------------------------------ local
+    def add(self, rows, scene_id, name=None, coords=None):
+        """Add one scene with its global id ``scene_id`` to this rank's shard; rows and coordinates are validated as in
+        ``SceneIndex.add``.  Local: no collective, no host synchronisation.  Returns ``scene_id``."""
+        if isinstance(scene_id, bool):
+            raise TypeError("ShardedSceneIndex.add: scene_id must be an integer")
+        try:
+            sid = operator.index(scene_id)
+        except TypeError:
+            raise TypeError(f"ShardedSceneIndex.add: scene_id must be an integer (got {type(scene_id).__name__})")
+        L = self.local
+        p = bisect.bisect_right(self._ids, sid)
+        s = L.add(rows, name=name, coords=coords)
+        if p < s:
+            self._move_last_scene(p)
+        self._ids.insert(p, sid)
+        self._dir = None
+        return sid
+
+    def _move_last_scene(self, p):
+        """the local index's last scene becomes local scene p; the scenes p .. move up by one"""
+        L = self.local
+        off, S = L._off, L.n_scenes
+        a, o, e = off[p], off[-2], off[-1]
+        n = e - o
+        for t in (L.rows, L.codes, L.row_exp, L.coords, L.row_scene):
+            if t is not None:
+                _rotate(t, a, o, e)
+        L.row_scene[a + n:e] += 1
+        L.row_scene[a:a + n].fill_(p)
+        L._off_dev[p + 1:S + 1] = L._off_dev[p:S] + n
+        L._off[:] = off[:p + 1] + [x + n for x in off[p:S]]
+        L.names.insert(p, L.names.pop())
+
+    # ------------------------------------------------------------------ directory
+    def sync(self):
+        """Build the directory (collective; one host synchronisation).  Raises the same ValueError on every rank when
+        the ids over the group are not exactly 0 .. S-1, or the widths or storages differ."""
+        L = self.local
+        rows = [b - a for a, b in zip(L._off[:-1], L._off[1:])]
+        with torch.cuda.device(self.device):
+            d = build_directory(self._ids, rows, L.names, L.channels, L.storage, self.group)
+            S, smax = len(d.owner), max(d.n_local)
+            dev = self.device
+            self._gid = torch.tensor(self._ids, dtype=torch.int64, device=dev)
+            self._base = torch.tensor(d.base if S else [0], dtype=torch.int64, device=dev)
+            self._place = torch.tensor([d.owner[g] * smax + d.local[g] for g in range(S)], dtype=torch.int64, device=dev)
+        self._smax = smax
+        self._dir = d
+
+    def _directory(self):
+        if self._dir is None:
+            raise RuntimeError("ShardedSceneIndex: the directory is out of date; call sync() on every rank")
+        return self._dir
+
+    @property
+    def n_scenes(self):
+        """scenes over the group, as of the last directory build"""
+        return len(self._directory().owner)
+
+    @property
+    def names(self):
+        """names by global id, as of the last directory build"""
+        return list(self._directory().names)
+
+    def owner(self, scene_id):
+        """the rank holding global scene ``scene_id``"""
+        d = self._directory()
+        if not 0 <= scene_id < len(d.owner):
+            raise IndexError(f"ShardedSceneIndex.owner: scene id {scene_id} outside 0 .. {len(d.owner) - 1}")
+        return d.owner[scene_id]
+
+    def _ready(self, what):
+        if self._dir is None:
+            self.sync()
+        if not self._dir.owner:
+            raise RuntimeError(f"ShardedSceneIndex.{what}: the index is empty")
+
+    # ------------------------------------------------------------------ merge helpers
+    def _gather(self, x):
+        """[world, *x.shape]: x of every rank"""
+        import torch.distributed as dist
+        out = [torch.empty_like(x) for _ in range(self.world)]
+        dist.all_gather(out, x.contiguous(), group=self.group)
+        return torch.stack(out)
+
+    def _keys(self, score, scene, row):
+        """global merge keys and global scene ids of decoded local results (osb_shard_keys)"""
+        d = self._dir
+        key, gsc = torch.empty_like(scene), torch.empty_like(scene)
+        C.call('osb_shard_keys', C.ptr(score.contiguous()), C.ptr(scene.contiguous()), C.ptr(row.contiguous()),
+               scene.numel(), C.ptr(self._gid) if self._gid.numel() else None, self._gid.numel(), C.ptr(self._base),
+               len(d.owner), sum(d.rows), C.ptr(key), C.ptr(gsc), C.stream_ptr())
+        return key, gsc
+
+    def _merge(self, keys):
+        """keys int64 [world, nq, m] -> winners int64 [nq, m], positions w * m + j (osb_shard_merge)"""
+        W, nq, m = keys.shape
+        win = torch.empty((nq, m), dtype=torch.int64, device=self.device)
+        C.call('osb_shard_merge', C.ptr(keys.contiguous()), W, nq, m, C.ptr(win), C.stream_ptr())
+        return win
+
+    @staticmethod
+    def _take(cols, win):
+        """cols [ncol, world, nq, m], winners [nq, m] -> [ncol, nq, m]"""
+        ncol, W, nq, m = cols.shape
+        flat = cols.permute(0, 2, 1, 3).reshape(ncol, nq, W * m)
+        return flat.gather(2, win.unsqueeze(0).expand(ncol, nq, m))
+
+    def _per_scene(self, cols):
+        """cols [ncol, world, smax, nq] -> [ncol, S, nq] in global id order"""
+        ncol, W, smax, nq = cols.shape
+        return cols.reshape(ncol, W * smax, nq).index_select(1, self._place)
+
+    def _pad_scenes(self, ts, nq):
+        """local per-scene tensors [S_r, nq] (int64) -> [ncol, smax, nq]"""
+        out = torch.zeros((len(ts), self._smax, nq), dtype=torch.int64, device=self.device)
+        for i, t in enumerate(ts):
+            out[i, :t.shape[0]] = t
+        return out
+
+    @staticmethod
+    def _bits(h):
+        return h.view(torch.int16).long()
+
+    @staticmethod
+    def _half(x):
+        return x.to(torch.int16).view(torch.float16)
+
+    # ------------------------------------------------------------------ collectives
+    def query(self, queries, k=1, threshold=None):
+        """``SceneIndex.query`` over the whole group (collective): a ``SearchResult`` whose ``scene`` is the global id and
+        whose per-scene outputs are [S, nq] by global id, equal bit for bit to the single index's.  With NCCL no host
+        synchronisation once the directory is built."""
+        if not 1 <= k <= MAX_K:
+            raise ValueError(f"ShardedSceneIndex.query: k={k} outside 1..{MAX_K}")
+        L = self.local
+        q = L._queries(queries, 'query')
+        nq = q.shape[0]
+        if nq > MAX_SHARD_QUERIES:
+            raise ValueError(f"ShardedSceneIndex.query: nq={nq} above {MAX_SHARD_QUERIES}; query in slices")
+        thr = None if threshold is None else L._thresholds(threshold, nq, 'query')
+        self._ready('query')
+        dev = self.device
+        with torch.cuda.device(dev):
+            if L.n_scenes:
+                res = L.query(q, k=k, threshold=thr)
+            else:
+                res = SearchResult(torch.full((nq, k), float('-inf'), dtype=torch.float16, device=dev),
+                                   torch.full((nq, k), -1, dtype=torch.int64, device=dev),
+                                   torch.full((nq, k), -1, dtype=torch.int64, device=dev),
+                                   torch.empty((0, nq), dtype=torch.float16, device=dev),
+                                   torch.empty((0, nq), dtype=torch.int64, device=dev),
+                                   None if thr is None else torch.empty((0, nq), dtype=torch.int64, device=dev))
+            key, gsc = self._keys(res.score, res.scene, res.row)
+            top = torch.stack([key, gsc, res.row, self._bits(res.score)])                      # [4, nq, k]
+            per = [self._bits(res.scene_max), res.scene_argmax] + ([] if thr is None else [res.scene_count])
+            per = self._pad_scenes(per, nq)                                                      # [ncol, smax, nq]
+            g = self._gather(torch.cat([top.reshape(-1), per.reshape(-1)]))
+            W = self.world
+            top_g = g[:, :top.numel()].reshape(W, 4, nq, k).transpose(0, 1)
+            win = self._merge(top_g[0])
+            dec = self._take(top_g[1:], win)
+            sc = self._per_scene(g[:, top.numel():].reshape(W, per.shape[0], self._smax, nq).transpose(0, 1))
+            return SearchResult(self._half(dec[2]), dec[0], dec[1], self._half(sc[0]), sc[1],
+                                None if thr is None else sc[2])
+
+    def regions(self, queries, threshold, max_regions=8, reach=1, min_voxels=1, hits=False, max_hits=2 ** 26):
+        """``SceneIndex.regions`` over the whole group (collective), equal bit for bit to the single index's: ranked
+        regions by global id, ``n_regions`` [S, nq], and with ``hits=True`` the hit list sorted by (query, global row),
+        ``hit_region`` the rank in the merged list.  Two host synchronisations, as the single index: one read of every
+        rank's hit totals (which size the hit gather; refused above ``max_hits`` summed over the group) and one read of
+        the status word OR-ed over the group.  Both refusals are raised on every rank."""
+        L = self.local
+        if L.coords is None:
+            raise RuntimeError("ShardedSceneIndex.regions: the index was built without coordinates (coords=True)")
+        if not 1 <= max_regions <= MAX_REGIONS:
+            raise ValueError(f"ShardedSceneIndex.regions: max_regions={max_regions} outside 1..{MAX_REGIONS}")
+        if reach not in (1, 2):
+            raise ValueError(f"ShardedSceneIndex.regions: reach={reach} outside 1..2")
+        if min_voxels < 1:
+            raise ValueError(f"ShardedSceneIndex.regions: min_voxels={min_voxels} below 1")
+        q = L._queries(queries, 'regions')
+        nq, dev, R, W = q.shape[0], self.device, int(max_regions), self.world
+        thr = L._thresholds(threshold, nq, 'regions')
+        self._ready('regions')
+        S, Sr, smax = self.n_scenes, L.n_scenes, self._smax
+        slices = [(i, q[i:i + MAX_QUERIES].contiguous(), thr[i:i + MAX_QUERIES].contiguous())
+                  for i in range(0, nq, MAX_QUERIES)]
+        with torch.cuda.device(dev):
+            counts = [L._query(qs, 1, ts).scene_count for _, qs, ts in slices] if Sr else None
+            mine = torch.stack([c.sum() for c in counts]) if Sr else torch.zeros(len(slices), dtype=torch.int64, device=dev)
+            totals = self._gather(mine).tolist()                                          # host sync 1
+        total = sum(map(sum, totals))
+        if total > max_hits:
+            raise RuntimeError(f"ShardedSceneIndex.regions: {total} hits over the group exceed max_hits={max_hits}; raise "
+                               f"the threshold or max_hits")
+        parts = []
+        with torch.cuda.device(dev):
+            status = torch.zeros(1, dtype=torch.int32, device=dev)
+            for si, (q0, qs, ts) in enumerate(slices):
+                m = qs.shape[0]
+                h = totals[self.rank][si]
+                out, hit_out, hsc = self._local_regions(qs, ts, counts[si] if Sr else None, h, R, reach, min_voxels,
+                                                        hits, status)
+                key, gsc = self._keys(out[0], out[1], out[2])
+                reg = torch.cat([torch.stack([key, gsc, out[2], out[3], self._bits(out[0])]),
+                                 out[4].long().permute(2, 0, 1), out[5].long().permute(2, 0, 1)])   # [11, m, R]
+                per = self._pad_scenes([out[6]], m)
+                flat = [reg.reshape(-1), per.reshape(-1)]
+                hmax = max(t[si] for t in totals)
+                if hits and hmax:
+                    hl = torch.zeros((7, hmax), dtype=torch.int64, device=dev)
+                    if h:
+                        hg = self._gid[hit_out[1]]
+                        hl[:, :h] = torch.stack([hit_out[0], self._base[hg] + hit_out[2], torch.full_like(hg, self.rank),
+                                                 hit_out[3], hg, hit_out[2], self._bits(hsc)])
+                    flat.append(hl.reshape(-1))
+                g = self._gather(torch.cat(flat))
+                n_reg, n_per = reg.numel(), per.numel()
+                reg_g = g[:, :n_reg].reshape(W, 11, m, R).transpose(0, 1)
+                win = self._merge(reg_g[0])
+                dec = self._take(reg_g[1:], win)
+                box = dec[4:].permute(1, 2, 0).to(torch.int32)                              # [m, R, 6]
+                n_regions = self._per_scene(g[:, n_reg:n_reg + n_per].reshape(W, 1, smax, m).transpose(0, 1))[0]
+                res = [self._half(dec[3]), dec[0], dec[1], dec[2], box[..., :3].contiguous(), box[..., 3:].contiguous(),
+                       n_regions]
+                if hits:
+                    H = sum(t[si] for t in totals)
+                    if H:
+                        hg_all = g[:, n_reg + n_per:].reshape(W, 7, hmax)
+                        hl = torch.cat([hg_all[w, :, :t[si]] for w, t in enumerate(totals) if t[si]], dim=1)
+                        order = torch.empty(H, dtype=torch.int64, device=dev)
+                        region = torch.empty(H, dtype=torch.int64, device=dev)
+                        ws_bytes = C.lib().osb_shard_hits_workspace_bytes(H)
+                        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+                        C.call('osb_shard_hits', C.ptr(hl[0].contiguous()), C.ptr(hl[1].contiguous()),
+                               C.ptr(hl[2].contiguous()), C.ptr(hl[3].contiguous()), H, W, m, R, C.ptr(win),
+                               C.ptr(order), C.ptr(region), C.ptr(ws), ws_bytes, C.stream_ptr())
+                        del ws
+                        hs = hl.index_select(1, order)
+                        res += [hs[0] + q0, hs[4], hs[5], self._half(hs[6]), region]
+                    else:
+                        res += [torch.empty(0, dtype=torch.int64, device=dev)] * 3 + \
+                               [torch.empty(0, dtype=torch.float16, device=dev),
+                                torch.empty(0, dtype=torch.int64, device=dev)]
+                else:
+                    res += [None] * 5
+                parts.append(res)
+            st = 0
+            for v in self._gather(status).reshape(-1).tolist():                          # host sync 2
+                st |= int(v)
+        if st & C_ST_RANGE:
+            raise RuntimeError("ShardedSceneIndex.regions: a hit's coordinate lies outside |x|, |y|, |z| < 2^17 - 256")
+        if st & C_ST_DUP:
+            raise RuntimeError("ShardedSceneIndex.regions: two hits of one (scene, query) share a voxel (duplicate "
+                               "coordinates)")
+        if st:
+            raise RuntimeError(f"ShardedSceneIndex.regions: the hit list does not match the search's counts (status {st})")
+        if len(parts) == 1:
+            return RegionResult(*parts[0])
+        cat = lambda j, d: None if parts[0][j] is None else torch.cat([p[j] for p in parts], dim=d)   # noqa: E731
+        return RegionResult(*[cat(j, 1 if j == 6 else 0) for j in range(12)])
+
+    def _local_regions(self, qs, ts, cnt, h, R, reach, min_voxels, hits, status):
+        """this rank's regions of one query slice, the steps of SceneIndex.regions: (region outputs with local scene
+        ids, local hit list (query, local scene, row, local region rank) or None, hit scores)"""
+        L, dev, m = self.local, self.device, qs.shape[0]
+        if not L.n_scenes:
+            out = [torch.full((m, R), float('-inf'), dtype=torch.float16, device=dev)] + \
+                  [torch.full((m, R), -1, dtype=torch.int64, device=dev) for _ in range(2)] + \
+                  [torch.zeros((m, R), dtype=torch.int64, device=dev)] + \
+                  [torch.zeros((m, R, 3), dtype=torch.int32, device=dev) for _ in range(2)] + \
+                  [torch.empty((0, m), dtype=torch.int64, device=dev)]
+            return out, None, None
+        S = L.n_scenes
+        if qs.data_ptr() % 16:
+            qs = qs.clone()
+        key = torch.empty(h, dtype=torch.int64, device=dev)
+        hsc = torch.empty(h, dtype=torch.float16, device=dev)
+        if h:
+            ws_bytes = C.lib().osb_search_hits_workspace_bytes(S, m, h)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+            sfx, operand = L._operand()
+            C.call('osb_search_hits' + sfx, *operand, C.ptr(L.row_scene), L.n_rows, L.channels,
+                   (C.I64 * (S + 1))(*L._off), S, C.ptr(qs), m, C.ptr(ts), C.ptr(cnt), h, C.ptr(key), C.ptr(hsc),
+                   C.ptr(status), C.ptr(ws), ws_bytes, C.stream_ptr())
+            del ws
+        out = [torch.empty((m, R), dtype=torch.float16, device=dev)] + \
+              [torch.empty((m, R), dtype=torch.int64, device=dev) for _ in range(3)] + \
+              [torch.empty((m, R, 3), dtype=torch.int32, device=dev) for _ in range(2)] + \
+              [torch.empty((S, m), dtype=torch.int64, device=dev)]
+        hit_out = [torch.empty(h, dtype=torch.int64, device=dev) for _ in range(4)] if hits else [None] * 4
+        ws_bytes = C.lib().osb_regions_workspace_bytes(h)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if h else None
+        C.call('osb_regions', C.ptr(key), C.ptr(hsc), h, C.ptr(L.coords), C.ptr(L.row_scene), C.ptr(L._off_dev),
+               L.n_rows, S, m, R, int(reach), int(min_voxels), *[C.ptr(t) for t in out], *[C.ptr(t) for t in hit_out],
+               C.ptr(status), C.ptr(ws), ws_bytes, C.stream_ptr())
+        return out, hit_out, hsc
 
 
 def regions_hit_bytes(n_hits, n_scenes, nq, hits=False):
