@@ -533,6 +533,37 @@ int osb_search_hits_f8(const void *codes_f8, const int8_t *row_exp, const int32_
                        const float *threshold, const int64_t *scene_count, int64_t n_hits, int64_t *hit_key,
                        void *hit_score_f16, int32_t *status, void *ws, size_t ws_bytes, void *stream);
 
+/* Labelled scene index (DESIGN.md, "Label contract").  row_label int64 / row_label_score fp16 [n_rows] are column 0 of
+ * osb_match_topk (topk = 1, normalize = 0, no point expansion) on the index's rows against a vocabulary of k_text classes.
+ * A query names m distinct classes classes_host int64 [m] (host memory, each in [0, k_text)); slot j stands for
+ * classes_host[j].  A row counts for slot j when its label is classes_host[j] and, with threshold fp32 [m], its label
+ * score is not NaN and float(score) >= threshold[j].
+ *
+ * osb_match_topk_f8: osb_match_topk (inds_reverse = NULL, normalize = 0) over FP8 index rows d = code * 2^e, codes
+ *   [n_rows, c] (16-byte aligned) and row_exp int8 [n_rows]; every output has the bits osb_match_topk gives on d.
+ * osb_label_counts: counts int64 [n_scenes, m] (overwritten) of the counted rows per scene and slot.  n_scenes * m at most
+ *   OSB_LABEL_MAX_COUNTS; threshold may be NULL (every row under its label counts, NaN scores included).  Workspace
+ *   osb_label_counts_workspace_bytes (8-byte aligned).
+ * osb_label_hits: the hit list of 1 <= m <= OSB_SEARCH_MAX_QUERIES slots in osb_search_hits' layout, which osb_regions
+ *   takes: hit_key int64 [n_hits] = (slot << 32) | global row, ascending; hit_score_f16 fp16 [n_hits] the label scores;
+ *   counts the osb_label_counts of the same classes and threshold (required), n_hits their sum; status or-ed with
+ *   OSB_REGIONS_ST_COUNT when a (slot, scene) segment does not receive exactly its count.  Workspace
+ *   osb_label_hits_workspace_bytes (8-byte aligned).
+ * Scene offsets are implied by row_scene int32 [n_rows] (non-decreasing, < n_scenes).  Class ids out of range or listed
+ * twice are refused on the host.  Integer atomics only: two calls give the same bits; no host synchronisation. */
+#define OSB_LABEL_MAX_COUNTS 134217728
+int osb_match_topk_f8(const void *codes_f8, const int8_t *row_exp, int64_t n_rows, int32_t c, const void *text_f16,
+                      int32_t k_text, int32_t topk, void *scores_f16, int64_t *label, float *smax, void *stream);
+size_t osb_label_counts_workspace_bytes(int32_t k_text, int32_t m);
+int osb_label_counts(const int64_t *row_label, const void *row_score_f16, const int32_t *row_scene, int64_t n_rows,
+                     int64_t n_scenes, int32_t k_text, const int64_t *classes_host, int32_t m, const float *threshold,
+                     int64_t *counts, void *ws, size_t ws_bytes, void *stream);
+size_t osb_label_hits_workspace_bytes(int32_t k_text, int64_t n_rows, int64_t n_scenes, int32_t m);
+int osb_label_hits(const int64_t *row_label, const void *row_score_f16, const int32_t *row_scene, int64_t n_rows,
+                   int64_t n_scenes, int32_t k_text, const int64_t *classes_host, int32_t m, const float *threshold,
+                   const int64_t *counts, int64_t n_hits, int64_t *hit_key, void *hit_score_f16, int32_t *status, void *ws,
+                   size_t ws_bytes, void *stream);
+
 /* Sharded scene index (DESIGN.md, "Sharded index contract"): the per-rank results of osb_search / osb_regions merged into
  * the results of one index holding every scene in ascending global id.  The directory maps each rank's local scene to its
  * global id (scene_gid int64 [n_local]) and each global id to its first global row (row_base int64 [n_global]).

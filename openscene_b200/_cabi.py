@@ -85,6 +85,11 @@ SIGNATURES = {
     'osb_index_quantize_f8': (c_int, [P, I32, I64, I32, P, P, P]),
     'osb_search_f8': (c_int, [P, P, P, I64, I32, P, P, I64, P, I32, I32, P, P, P, P, P, P, P, P, SZ, P]),
     'osb_search_hits_f8': (c_int, [P, P, P, I64, I32, P, I64, P, I32, P, P, I64, P, P, P, P, SZ, P]),
+    'osb_match_topk_f8': (c_int, [P, P, I64, I32, P, I32, I32, P, P, P, P]),
+    'osb_label_counts_workspace_bytes': (SZ, [I32, I32]),
+    'osb_label_counts': (c_int, [P, P, P, I64, I64, I32, P, I32, P, P, P, SZ, P]),
+    'osb_label_hits_workspace_bytes': (SZ, [I32, I64, I64, I32]),
+    'osb_label_hits': (c_int, [P, P, P, I64, I64, I32, P, I32, P, P, I64, P, P, P, P, SZ, P]),
     'osb_shard_keys': (c_int, [P, P, P, I64, P, I64, P, I64, I64, P, P, P]),
     'osb_shard_merge': (c_int, [P, I32, I32, I32, P, P]),
     'osb_shard_hits_workspace_bytes': (SZ, [I64]),

@@ -150,7 +150,8 @@ int match_tc_ce_run(const void *feat, int feat_is_f16, int c, const int64_t *ind
                     void *loss_f16, uint64_t *areas, int32_t *bad, void *ws, cudaStream_t stream);
 int match_tc_topk_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
                       const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize, int topk,
-                      void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, cudaStream_t stream);
+                      void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, const int8_t *row_exp,
+                      cudaStream_t stream);
 // CUDA-core repeat vote (vote.cu)
 int vote_accumulate_run(const void *src, int src_is_f16, const int64_t *inds_reverse, int64_t n_pts, int k, void *store,
                         int64_t *label_cur, int64_t *label_acc, cudaStream_t stream);
@@ -314,7 +315,19 @@ int osb_match_topk(const void *feat, int32_t feat_is_f16, int64_t n_vox, int32_t
   OSB_CHECK(feat != nullptr, "osb_match_topk: NULL features");
   if (n_pts == 0) return 0;
   return match_tc_topk_run(feat, feat_is_f16, nullptr, nullptr, nullptr, c, inds_reverse, n_pts, text_f16, k_text, normalize,
-                           topk, scores_f16, label, smax, nullptr, (cudaStream_t)stream_);
+                           topk, scores_f16, label, smax, nullptr, nullptr, (cudaStream_t)stream_);
+}
+
+// osb_match_topk over FP8 scene-index rows d = code * 2^e (no point expansion, no normalisation)
+int osb_match_topk_f8(const void *codes_f8, const int8_t *row_exp, int64_t n_rows, int32_t c, const void *text_f16,
+                      int32_t k_text, int32_t topk, void *scores_f16, int64_t *label, float *smax, void *stream_) {
+  if (check_topk_args("osb_match_topk_f8", c, k_text, topk, n_rows, n_rows, text_f16, label)) return 1;
+  OSB_CHECK(codes_f8 != nullptr && row_exp != nullptr, "osb_match_topk_f8: NULL codes or row exponents");
+  OSB_CHECK(n_rows < (int64_t(1) << 31), "osb_match_topk_f8: N=%lld outside 1..2^31-1", (long long)n_rows);
+  OSB_CHECK(((uintptr_t)codes_f8 & 15) == 0 && ((uintptr_t)text_f16 & 15) == 0,
+            "osb_match_topk_f8: codes and text must be 16-byte aligned");
+  return match_tc_topk_run(codes_f8, 1, nullptr, nullptr, nullptr, c, nullptr, n_rows, text_f16, k_text, 0, topk,
+                           scores_f16, label, smax, nullptr, row_exp, (cudaStream_t)stream_);
 }
 
 int osb_match_ensemble_topk(const float *feat3d, const void *feat2d_f16, int64_t n_vox, int32_t c,
@@ -325,7 +338,7 @@ int osb_match_ensemble_topk(const float *feat3d, const void *feat2d_f16, int64_t
   OSB_CHECK(feat3d && feat2d_f16 && sel_a && sel_b, "osb_match_ensemble_topk: NULL features or row maxima");
   if (n_pts == 0) return 0;
   return match_tc_topk_run(feat3d, 0, feat2d_f16, sel_a, sel_b, c, inds_reverse, n_pts, text_f16, k_text, 0, topk, scores_f16,
-                           label, nullptr, feat_out_f16, (cudaStream_t)stream_);
+                           label, nullptr, feat_out_f16, nullptr, (cudaStream_t)stream_);
 }
 
 }  // extern "C"

@@ -24,7 +24,9 @@
 //
 // k_match_tc_topk is the same kernel with a running per-point top-k (k <= 8) in the epilogue (MatchTcTopk below), so the
 // number of passes has no bound of its own: the result is [N_pts, k], never [N_pts, K].  The three kernels above compile
-// to the same instructions as before it existed.
+// to the same instructions as before it existed.  k_match_tc_topk<NP, true> takes its A tile from the FP8 scene index
+// (mt_fill_a8: e4m3 codes and per-row exponents, the tile mt_fill_a writes for the rows d), which labels the index
+// (search.py, SceneIndex.label) with the bits the fp16 kernel gives on d.
 #include "match_tc.cuh"
 #include "metric.cuh"
 #include "vote.cuh"
@@ -64,6 +66,7 @@ struct MatchTcTopk {
   int k;                             // 1..8, at most K
   __half *scores;                    // [n_pts, k] or NULL
   int64_t *label;                    // [n_pts, k]
+  const int8_t *row_exp;             // [n_pts] (k_match_tc_topk<NP, true>): p.feat holds e4m3 codes [n_pts, C]
 };
 constexpr int MT_TOPK_MAX = 8;
 
@@ -78,7 +81,7 @@ __device__ __forceinline__ int ce_label(const MatchTcCe &ce, int64_t pt, int64_t
   return ce.ignore == -1 ? -2 : -1;
 }
 
-template <int NP, int MODE>   // half2 pairs per lane: C = 64 * NP
+template <int NP, int MODE, bool F8 = false>   // half2 pairs per lane: C = 64 * NP
 __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const MatchTcParams p, const MatchTcVote vo,
                                               const MatchTcCe ce, const MatchTcTopk tk) {
   constexpr bool VOTE = MODE == MT_VOTE, CE = MODE == MT_CE, TOPK = MODE == MT_TOPK;
@@ -114,7 +117,10 @@ __device__ __forceinline__ void match_tc_body(const CUtensorMap &tmT, const Matc
 
   if (warp < MT_PW) {
     // ============================ A producers: 8 rows per warp ==============================
-    mt_fill_a<NP>(p, sA, row0, warp, lane);
+    if constexpr (F8)
+      mt_fill_a8<NP>(reinterpret_cast<const uint8_t *>(p.feat), tk.row_exp, p.n_pts, sA, row0, warp, lane);
+    else
+      mt_fill_a<NP>(p, sA, row0, warp, lane);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic-proxy writes -> wgmma reads
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a_full) : "memory");
   } else if (warp == MT_PW) {
@@ -425,10 +431,10 @@ k_match_tc_ce(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, co
   match_tc_body<NP, MT_CE>(tmT, p, MatchTcVote{}, ce, MatchTcTopk{});
 }
 
-template <int NP>
+template <int NP, bool F8 = false>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 k_match_tc_topk(const __grid_constant__ CUtensorMap tmT, const MatchTcParams p, const MatchTcTopk tk) {
-  match_tc_body<NP, MT_TOPK>(tmT, p, MatchTcVote{}, MatchTcCe{}, tk);
+  match_tc_body<NP, MT_TOPK, F8>(tmT, p, MatchTcVote{}, MatchTcCe{}, tk);
 }
 
 static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, const MatchTcCe *ce, const MatchTcTopk *tk,
@@ -440,7 +446,13 @@ static int launch_match_tc(const MatchTcParams &p, const MatchTcVote *vote, cons
   const unsigned grid = (unsigned)ceil_div(p.n_pts, MT_M);
   if (tk != nullptr) {
     const size_t smem_tk = smem + (size_t)MT_M * MT_TOPK_MAX * 8;   // + the lists
-    if (NP == 12) {
+    if (tk->row_exp && NP == 12) {
+      OSB_SMEM_ATTR_ONCE((k_match_tc_topk<12, true>), 227 * 1024);
+      k_match_tc_topk<12, true><<<grid, MT_THREADS, smem_tk, stream>>>(tmT, p, *tk);
+    } else if (tk->row_exp) {
+      OSB_SMEM_ATTR_ONCE((k_match_tc_topk<8, true>), 227 * 1024);
+      k_match_tc_topk<8, true><<<grid, MT_THREADS, smem_tk, stream>>>(tmT, p, *tk);
+    } else if (NP == 12) {
       OSB_SMEM_ATTR_ONCE(k_match_tc_topk<12>, 227 * 1024);
       k_match_tc_topk<12><<<grid, MT_THREADS, smem_tk, stream>>>(tmT, p, *tk);
     } else {
@@ -537,13 +549,14 @@ int match_tc_ce_run(const void *feat, int feat_is_f16, int c, const int64_t *ind
   return launch_match_tc(p, nullptr, &ce, nullptr, text_f16, stream);
 }
 
-// streaming top-k: any number of passes (the caller bounds K)
+// streaming top-k: any number of passes (the caller bounds K); row_exp non-NULL: feat holds e4m3 codes (FP8 index rows)
 int match_tc_topk_run(const void *feat, int feat_is_f16, const void *feat2_f16, const float *sel_a, const float *sel_b, int c,
                       const int64_t *inds_reverse, int64_t n_pts, const void *text_f16, int k_text, int normalize, int topk,
-                      void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, cudaStream_t stream) {
+                      void *scores_f16, int64_t *label, float *smax, void *feat_out_f16, const int8_t *row_exp,
+                      cudaStream_t stream) {
   const MatchTcParams p = match_tc_params(feat, feat_is_f16, feat2_f16, sel_a, sel_b, c, inds_reverse, n_pts, k_text,
                                           normalize, nullptr, nullptr, smax, feat_out_f16);
-  const MatchTcTopk tk{topk, (__half *)scores_f16, label};
+  const MatchTcTopk tk{topk, (__half *)scores_f16, label, row_exp};
   return launch_match_tc(p, nullptr, nullptr, &tk, text_f16, stream);
 }
 

@@ -312,6 +312,14 @@ k_hit_segments(const int64_t *__restrict__ scene_count, int64_t n_scenes, int nq
   }
 }
 
+// the segments of a hit list whose counts [S][nq] are known (label.cu's class hits), as osb_search_hits lays them out
+int hit_segments_run(const int64_t *scene_count, int64_t n_scenes, int nq, int64_t n_hits, unsigned long long *cursor,
+                     unsigned long long *seg_end, int *status, cudaStream_t stream) {
+  k_hit_segments<<<1, 1024, 0, stream>>>(scene_count, n_scenes, nq, n_hits, cursor, seg_end, status);
+  OSB_LAUNCH_CHECK();
+  return 0;
+}
+
 // every segment received exactly its count; the scores follow the sorted keys (payload = arrival slot)
 __global__ void k_hit_finish(const unsigned long long *__restrict__ cursor, const unsigned long long *__restrict__ seg_end,
                              int64_t n_seg, const int32_t *__restrict__ slot, const __half *__restrict__ score_in,

@@ -19,6 +19,11 @@ An index built with ``storage='fp8'`` keeps each row as e4m3 codes and one power
 2 C; DESIGN.md, "FP8 index contract"): twice the rows in the same memory, and each query slice reads half the bytes.  It
 answers exactly what an fp16 index holding the dequantized rows answers.
 
+``label`` labels every row against a vocabulary, as OpenScene segments a scene (the argmax over the label set), and keeps
+the labels current through later adds (csrc/label.cu; DESIGN.md, "Label contract"): ``labels`` gives a scene's
+segmentation, ``class_counts`` the rows of each class per scene, and ``class_regions`` the connected pieces of each
+class (zero-shot instance proposals) through the same region grower as ``regions``.
+
 ``ShardedSceneIndex`` spreads one database over the ranks of a process group (csrc/shard.cu; DESIGN.md, "Sharded index
 contract"): each rank keeps the scenes it computed, a query runs ``k_search`` on every shard, and the small per-shard
 results are merged on the device after one collective.  Every output is bit for bit the output of one ``SceneIndex``
@@ -35,6 +40,8 @@ from . import _cabi as C
 MAX_QUERIES = 96      # OSB_SEARCH_MAX_QUERIES: one 96-column wgmma pass per launch
 MAX_K = 32            # OSB_SEARCH_MAX_K
 MAX_REGIONS = 32      # OSB_REGIONS_MAX_R
+MAX_VOCAB = 1 << 20   # OSB_MATCH_TOPK_MAX_TEXT
+MAX_COUNTS = 1 << 27  # OSB_LABEL_MAX_COUNTS
 C_ST_COUNT, C_ST_RANGE, C_ST_DUP = 1, 2, 4      # OSB_REGIONS_ST_*: the status word of osb_search_hits / osb_regions
 
 SearchResult = namedtuple('SearchResult', 'score scene row scene_max scene_argmax scene_count')
@@ -88,6 +95,7 @@ class SceneIndex:
         self._off = [0]                                    # host offsets, n_scenes + 1
         self._off_dev = torch.zeros(64, dtype=torch.int64, device=self.device)
         self.names = []
+        self.vocab = self.row_label = self.row_label_score = None       # set by label()
 
     @property
     def n_rows(self):
@@ -169,9 +177,168 @@ class SceneIndex:
             grown[:self._off_dev.numel()].copy_(self._off_dev)
             self._off_dev = grown
         self._off_dev[s + 1:s + 2].fill_(o + n)           # a fill kernel, not a copy from host memory
+        if self.vocab is not None:
+            self._label_rows(o, o + n)
         self._off.append(o + n)
         self.names.append(name)
         return s
+
+    # ------------------------------------------------------------------ labels (DESIGN.md, "Label contract")
+    def label(self, vocab):
+        """Label every row against a vocabulary (fp16 / fp32 [K, C], 1 <= K <= 2^20; fp32 is taken as ``.half()``): the
+        label of row r is column 0 of ``osb_match_topk(topk=1)`` on the row, the first NaN else the first maximum with
+        -0 == +0, which on NaN-free rows is ``evaluate.py``'s ``torch.max(pred, 1)[1]``; its fp16 score is kept with it.
+        An FP8 index labels the rows d it stands for (``osb_match_topk_f8``).  The first call allocates ``row_label``
+        (int64) and ``row_label_score`` (fp16) over the capacity, 10 B per row.  The index keeps a copy of the
+        vocabulary, and every later ``add`` labels its scene in the same call, so every row always carries its label
+        under the current vocabulary; calling ``label`` again replaces the vocabulary and every label.  One launch, no
+        host synchronisation; on an empty index only the vocabulary is stored."""
+        if not isinstance(vocab, torch.Tensor) or vocab.dim() != 2:
+            raise ValueError("SceneIndex.label: vocab must be a 2-D tensor [K, C]")
+        if vocab.dtype not in (torch.float16, torch.float32):
+            raise TypeError(f"SceneIndex.label: vocab must be fp16 or fp32 (got {vocab.dtype})")
+        if vocab.device != self.device:
+            raise ValueError(f"SceneIndex.label: vocab is on {vocab.device}, the index on {self.device}")
+        K, c = vocab.shape
+        if c != self.channels:
+            raise ValueError(f"SceneIndex.label: vocab has width {c}, the index {self.channels}")
+        if not 1 <= K <= MAX_VOCAB:
+            raise ValueError(f"SceneIndex.label: {K} classes outside 1..{MAX_VOCAB}")
+        with torch.cuda.device(self.device):
+            self.vocab = vocab.to(torch.float16, copy=True).contiguous()
+            if self.row_label is None:
+                self.row_label = torch.empty(self.capacity, dtype=torch.int64, device=self.device)
+                self.row_label_score = torch.empty(self.capacity, dtype=torch.float16, device=self.device)
+        if self.n_rows:
+            self._label_rows(0, self.n_rows)
+
+    def _label_rows(self, a, b):
+        K = self.vocab.shape[0]
+        with torch.cuda.device(self.device):
+            if self.codes is None:
+                C.call('osb_match_topk', C.ptr(self.rows[a:b]), 1, b - a, self.channels, None, b - a, C.ptr(self.vocab),
+                       K, 0, 1, C.ptr(self.row_label_score[a:b]), C.ptr(self.row_label[a:b]), None, C.stream_ptr())
+            else:
+                C.call('osb_match_topk_f8', C.ptr(self.codes[a:b]), C.ptr(self.row_exp[a:b]), b - a, self.channels,
+                       C.ptr(self.vocab), K, 1, C.ptr(self.row_label_score[a:b]), C.ptr(self.row_label[a:b]), None,
+                       C.stream_ptr())
+
+    def _labelled(self, what):
+        if self.vocab is None:
+            raise RuntimeError(f"SceneIndex.{what}: the index is not labelled; call label(vocab) first")
+        return self.vocab.shape[0]
+
+    def labels(self, scene):
+        """The labels (int64 [n]) and label scores (fp16 [n]) of one scene, row for row with ``scene_rows`` (views)."""
+        self._labelled('labels')
+        a, b = self._off[scene], self._off[scene + 1]
+        return self.row_label[a:b], self.row_label_score[a:b]
+
+    def _classes(self, classes, K, what):
+        """a host sequence of distinct class ids in [0, K) -> list of ints (refused before any launch)"""
+        if isinstance(classes, torch.Tensor):
+            if classes.device.type != 'cpu' or classes.dim() != 1 or classes.dtype.is_floating_point or \
+                    classes.dtype == torch.bool:
+                raise ValueError(f"SceneIndex.{what}: classes must be a 1-D integer CPU tensor or a host sequence")
+            ids = [int(v) for v in classes.tolist()]
+        else:
+            if isinstance(classes, (str, bytes)) or not hasattr(classes, '__iter__'):
+                raise ValueError(f"SceneIndex.{what}: classes must be a sequence of class ids")
+            ids = []
+            for v in classes:
+                if isinstance(v, bool):
+                    raise ValueError(f"SceneIndex.{what}: class ids must be integers (got {v!r})")
+                try:
+                    ids.append(operator.index(v))
+                except TypeError:
+                    raise ValueError(f"SceneIndex.{what}: class ids must be integers (got {v!r})")
+        if not ids:
+            raise ValueError(f"SceneIndex.{what}: no classes")
+        bad = [v for v in ids if not 0 <= v < K]
+        if bad:
+            raise ValueError(f"SceneIndex.{what}: class {bad[0]} outside 0..{K - 1}")
+        if len(set(ids)) != len(ids):
+            seen = set()
+            dup = next(v for v in ids if v in seen or seen.add(v))
+            raise ValueError(f"SceneIndex.{what}: class {dup} listed twice")
+        return ids
+
+    def _class_thresholds(self, threshold, m, what):
+        """a float, [m] values or a tensor -> fp32 [m] on the device, without a host synchronisation: host values go
+        through pinned memory and an asynchronous copy"""
+        if isinstance(threshold, torch.Tensor) and threshold.is_cuda:
+            thr = threshold.to(device=self.device, dtype=torch.float32).reshape(-1)
+        elif isinstance(threshold, (int, float)) and not isinstance(threshold, bool):
+            thr = torch.full((1,), float(threshold), dtype=torch.float32, device=self.device)
+        else:
+            host = torch.as_tensor(threshold, dtype=torch.float32).reshape(-1)
+            thr = host.pin_memory().to(self.device, non_blocking=True)
+        if thr.numel() == 1:
+            thr = thr.expand(m)
+        if thr.numel() != m:
+            raise ValueError(f"SceneIndex.{what}: {thr.numel()} thresholds for {m} classes")
+        return thr.contiguous()
+
+    def _label_counts(self, ids, thr):
+        """osb_label_counts: int64 [S, len(ids)]"""
+        S, dev, m = self.n_scenes, self.device, len(ids)
+        with torch.cuda.device(dev):
+            cnt = torch.empty((S, m), dtype=torch.int64, device=dev)
+            ws_bytes = C.lib().osb_label_counts_workspace_bytes(self.vocab.shape[0], m)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+            C.call('osb_label_counts', C.ptr(self.row_label), C.ptr(self.row_label_score), C.ptr(self.row_scene),
+                   self.n_rows, S, self.vocab.shape[0], (C.I64 * m)(*ids), m, C.ptr(thr), C.ptr(cnt), C.ptr(ws),
+                   ws_bytes, C.stream_ptr())
+        return cnt
+
+    def class_counts(self, classes=None, threshold=None):
+        """Per scene, the rows labelled each class: int64 [S, m], m = len(classes) (default: all K classes in order).
+        Without ``threshold`` every row counts under its label, NaN scores included (the segmentation ``evaluate.py``
+        counts); with ``threshold`` (a float or [m] values) only rows whose label score is not NaN and at or above
+        threshold[j].  Refused above 2^27 counts.  No host synchronisation."""
+        K = self._labelled('class_counts')
+        ids = list(range(K)) if classes is None else self._classes(classes, K, 'class_counts')
+        m, S = len(ids), self.n_scenes
+        if S * m > MAX_COUNTS:
+            raise ValueError(f"SceneIndex.class_counts: {S} scenes x {m} classes exceed {MAX_COUNTS} counts")
+        thr = None if threshold is None else self._class_thresholds(threshold, m, 'class_counts')
+        if S == 0:
+            return torch.zeros((0, m), dtype=torch.int64, device=self.device)
+        return self._label_counts(ids, thr)
+
+    def class_regions(self, classes, threshold=None, max_regions=8, reach=1, min_voxels=1, hits=False, max_hits=2 ** 26):
+        """``regions`` over the labels: the hits of class slot j are the rows labelled classes[j] whose label score is
+        not NaN and at or above threshold[j] (default -inf), grouped into connected regions as ``regions`` groups them
+        and ranked by the search key of their best hit.  Returns a ``RegionResult`` whose query axis is the position in
+        ``classes``; any number of classes, in slices of 96.  Two host synchronisations, as ``regions``: the total hit
+        count (refused above ``max_hits`` before the hit list is allocated) and the status word."""
+        K = self._labelled('class_regions')
+        if self.coords is None:
+            raise RuntimeError("SceneIndex.class_regions: the index was built without coordinates (coords=True)")
+        if self.n_scenes == 0:
+            raise RuntimeError("SceneIndex.class_regions: the index is empty")
+        if not 1 <= max_regions <= MAX_REGIONS:
+            raise ValueError(f"SceneIndex.class_regions: max_regions={max_regions} outside 1..{MAX_REGIONS}")
+        if reach not in (1, 2):
+            raise ValueError(f"SceneIndex.class_regions: reach={reach} outside 1..2")
+        if min_voxels < 1:
+            raise ValueError(f"SceneIndex.class_regions: min_voxels={min_voxels} below 1")
+        ids = self._classes(classes, K, 'class_regions')
+        m, S, dev, R = len(ids), self.n_scenes, self.device, int(max_regions)
+        thr = self._class_thresholds(float('-inf') if threshold is None else threshold, m, 'class_regions')
+        slices = [(i, ids[i:i + MAX_QUERIES], thr[i:i + MAX_QUERIES].contiguous()) for i in range(0, m, MAX_QUERIES)]
+        counts = [self._label_counts(ci, ts) for _, ci, ts in slices]
+
+        def emit(si, h, cnt, key, hsc, status):
+            _, ci, ts = slices[si]
+            ws_bytes = C.lib().osb_label_hits_workspace_bytes(K, self.n_rows, S, len(ci))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+            C.call('osb_label_hits', C.ptr(self.row_label), C.ptr(self.row_label_score), C.ptr(self.row_scene),
+                   self.n_rows, S, K, (C.I64 * len(ci))(*ci), len(ci), C.ptr(ts), C.ptr(cnt), h, C.ptr(key), C.ptr(hsc),
+                   C.ptr(status), C.ptr(ws), ws_bytes, C.stream_ptr())
+
+        return self._grow('class_regions', 'the label counts', [(q0, len(ci)) for q0, ci, _ in slices], counts, emit,
+                          R, reach, min_voxels, hits, max_hits)
 
     def query(self, queries, k=1, threshold=None):
         """Score queries (fp16/fp32 [nq, C] or [C]) against every row.  ``threshold`` (float or [nq]) turns on the
@@ -261,30 +428,40 @@ class SceneIndex:
         slices = [(i, q[i:i + MAX_QUERIES].contiguous(), thr[i:i + MAX_QUERIES].contiguous())
                   for i in range(0, nq, MAX_QUERIES)]
         counts = [self._query(qs, 1, ts).scene_count for _, qs, ts in slices]
+
+        def emit(si, h, cnt, key, hsc, status):
+            _, qs, ts = slices[si]
+            if qs.data_ptr() % 16:
+                qs = qs.clone()
+            ws_bytes = C.lib().osb_search_hits_workspace_bytes(S, qs.shape[0], h)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+            sfx, operand = self._operand()
+            C.call('osb_search_hits' + sfx, *operand, C.ptr(self.row_scene), self.n_rows, self.channels,
+                   (C.I64 * (S + 1))(*self._off), S, C.ptr(qs), qs.shape[0], C.ptr(ts), C.ptr(cnt), h, C.ptr(key),
+                   C.ptr(hsc), C.ptr(status), C.ptr(ws), ws_bytes, C.stream_ptr())
+
+        return self._grow('regions', "the search's counts", [(q0, qs.shape[0]) for q0, qs, _ in slices], counts, emit,
+                          R, reach, min_voxels, hits, max_hits)
+
+    def _grow(self, what, counted_by, slices, counts, emit, R, reach, min_voxels, hits, max_hits):
+        """The tail of ``regions`` and ``class_regions``: per slice (q0, m) with counts [S, m], read the hit totals (host
+        sync 1), refuse above max_hits, allocate the hit list, fill it with emit(slice, n_hits, counts, key, score,
+        status), grow the regions with ``osb_regions``, and read the status word (host sync 2)."""
+        S, dev = self.n_scenes, self.device
         with torch.cuda.device(dev):
             totals = [int(t) for t in torch.stack([c.sum() for c in counts]).tolist()]      # host sync 1
         total = sum(totals)
         if total > max_hits:
-            raise RuntimeError(f"SceneIndex.regions: {total} hits exceed max_hits={max_hits}; raise the threshold or "
+            raise RuntimeError(f"SceneIndex.{what}: {total} hits exceed max_hits={max_hits}; raise the threshold or "
                                f"max_hits")
-        off_host = (C.I64 * (S + 1))(*self._off)
         parts = []
         with torch.cuda.device(dev):
             status = torch.zeros(1, dtype=torch.int32, device=dev)
-            for (q0, qs, ts), cnt, h in zip(slices, counts, totals):
-                m = qs.shape[0]
-                if qs.data_ptr() % 16:
-                    qs = qs.clone()
+            for si, ((q0, m), cnt, h) in enumerate(zip(slices, counts, totals)):
                 key = torch.empty(h, dtype=torch.int64, device=dev)
                 hsc = torch.empty(h, dtype=torch.float16, device=dev)
                 if h:
-                    ws_bytes = C.lib().osb_search_hits_workspace_bytes(S, m, h)
-                    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-                    sfx, operand = self._operand()
-                    C.call('osb_search_hits' + sfx, *operand, C.ptr(self.row_scene), self.n_rows, self.channels,
-                           off_host, S, C.ptr(qs), m, C.ptr(ts), C.ptr(cnt), h, C.ptr(key), C.ptr(hsc), C.ptr(status),
-                           C.ptr(ws), ws_bytes, C.stream_ptr())
-                    del ws
+                    emit(si, h, cnt, key, hsc, status)
                 out = [torch.empty((m, R), dtype=torch.float16, device=dev)] + \
                       [torch.empty((m, R), dtype=torch.int64, device=dev) for _ in range(3)] + \
                       [torch.empty((m, R, 3), dtype=torch.int32, device=dev) for _ in range(2)] + \
@@ -303,14 +480,14 @@ class SceneIndex:
                     parts.append(out + [None] * 5)
             st = int(status.item())                                                         # host sync 2
         if st & C_ST_RANGE:
-            raise RuntimeError("SceneIndex.regions: a hit's coordinate lies outside |x|, |y|, |z| < 2^17 - 256")
+            raise RuntimeError(f"SceneIndex.{what}: a hit's coordinate lies outside |x|, |y|, |z| < 2^17 - 256")
         if st & C_ST_DUP:
-            raise RuntimeError("SceneIndex.regions: two hits of one (scene, query) share a voxel (duplicate coordinates)")
+            raise RuntimeError(f"SceneIndex.{what}: two hits of one (scene, query) share a voxel (duplicate coordinates)")
         if st:
-            raise RuntimeError(f"SceneIndex.regions: the hit list does not match the search's counts (status {st})")
+            raise RuntimeError(f"SceneIndex.{what}: the hit list does not match {counted_by} (status {st})")
         if len(parts) == 1:
             return RegionResult(*parts[0])
-        cat = lambda j, d: None if parts[0][j] is None else torch.cat([p[j] for p in parts], dim=d)
+        cat = lambda j, d: None if parts[0][j] is None else torch.cat([p[j] for p in parts], dim=d)   # noqa: E731
         return RegionResult(*[cat(j, 1 if j == 6 else 0) for j in range(12)])
 
     def _query(self, q, k, thr):
